@@ -44,7 +44,7 @@ static std::atomic<long long> g_launches{0};       // instrumentation only (mage
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize belongs to (function, device), not to an engine: it is only ever raised,
 // under a lock, so that a second engine with a smaller need cannot pull it from under the first
-enum { ATTR_STEP = 0, ATTR_OBS0 = 1, ATTR_N = 1 + 8, ATTR_MAX_DEVICES = 64 };
+enum { ATTR_STEP = 0, ATTR_OBS0 = 1, ATTR_N = 1 + 12, ATTR_MAX_DEVICES = 64 };
 static std::mutex g_attr_mu;
 static size_t g_attr_smem[ATTR_MAX_DEVICES][ATTR_N];
 template <class K>
@@ -72,7 +72,7 @@ struct Ctx {
     // per-observer headers of the render kernel
     int4 *obs_hdr = nullptr; size_t obs_hdr_n = 0;
     // cudaFuncSetAttribute caches (per device: a context never changes device)
-    struct ObsCfg { size_t smem = (size_t)-1; int ctas_per_sm = 1; } obs_cfg[8];
+    struct ObsCfg { size_t smem = (size_t)-1; int ctas_per_sm = 1; } obs_cfg[12];
     int *pin_done = nullptr; size_t pin_done_n = 0;         // pinned read-back of EngineDev::done
     int *pin_counts = nullptr; size_t pin_counts_n = 0;     // pinned read-back of EngineDev::off (clear_dead)
     cudaEvent_t ev_counts = nullptr;
@@ -850,9 +850,9 @@ void launch_obs_prepare(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsign
 // a handful of values gathered from the map.  Two ceilings matter: the TMA bulk-store stream itself and the L2
 // throughput summed over reads and writes -- so every byte the kernel READS through L2 competes with the bytes it
 // writes:
-//   * tile = TA (4) consecutive agents of the ABI concatenation = ONE 128-thread CTA, one warp per agent, one
-//     shared-memory tile (18.9 KB for battle), 8 CTAs = 32 warps per SM, tiles dealt round-robin so the whole
-//     grid works inside a window of a few arenas (their planes / minimaps stay L1/L2-hot);
+//   * tile = TA consecutive agents of the ABI concatenation = ONE CTA of TA warps, one warp per agent, one
+//     shared-memory tile, 32 warps per SM (battle f32: 8 agents, 37.9 KB, 4 CTAs per SM), tiles dealt round-robin so
+//     the whole grid works inside a window of a few arenas (their planes / minimaps stay L1/L2-hot);
 //   * the map is gathered from a ONE-BYTE kind plane (0 empty / 1 wall / 2+group; a view row is one 32-byte
 //     sector) and only occupied cells (~5 %) take a second, dependent load from the hp_norm plane;
 //   * the tile is composed entirely on the SM: each warp zero-fills its own record, copies the arena's
@@ -861,25 +861,24 @@ void launch_obs_prepare(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsign
 //     no template tile is read through L2;
 //   * the tile leaves the SM as ONE TMA bulk STORE (cp.async.bulk.global.shared::cta, SASS UBLKCP).  A tile's
 //     byte range in the output is contiguous and 16-byte aligned because TA * sizeof(T) % 16 == 0.
+//   * two tile widths (launch_obs_typed picks one per launch): the wide tile (8 f32 / 16 f16 agents) is 32 bytes
+//     per record element, so its byte range is also 32-byte aligned for any record length -- a tile that starts
+//     or ends inside a 32-byte sector shares that sector with a tile of another CTA.  It is used whenever it keeps
+//     at least as many warps per SM as the narrow tile (4 f32 / 8 f16 agents), which also serves records too large
+//     for a wide tile in shared memory.
 // Algorithmic traffic per agent: sizeof(T)*(view_h*view_w*n_channel + feature) bytes written, plus one compulsory
 // read of the occupancy plane per arena (DESIGN.md section 6).  No tensor cores: there is no contraction here.
-#ifndef OBS_TA_N
-#define OBS_TA_N 4
-#endif
 #ifndef OBS_ABLATE
 #define OBS_ABLATE 0                 // profiling experiments only: 1 no plane gather, 2 no tile
 #endif                               // init (zero + minimap), 4 no feature rows, 8 no bulk store -- results are WRONG
 
 // output element type of the observation: float = the reference ABI (env_get_observation); __half = the compact
 // hand-off format of magent_b200_get_observation_f16 (each value is the f32 value rounded to nearest-even).
-// TA = agents per tile = warps per CTA; TA * sizeof(T) % 16 == 0 keeps every tile's byte range 16-byte aligned.
 template <typename T> struct ObsOut;
 template <> struct ObsOut<float> {
-    static constexpr int TA = OBS_TA_N;
     static __device__ __forceinline__ float cv(float v) { return v; }
 };
 template <> struct ObsOut<__half> {
-    static constexpr int TA = 2 * OBS_TA_N;
     static __device__ __forceinline__ __half cv(float v) {
         if (v != v) {                    // keep sign and top payload bits like a software f32->f16 cast does (numpy astype)
             const unsigned u = __float_as_uint(v);
@@ -976,14 +975,23 @@ __global__ void __launch_bounds__(256) obs_headers_kernel(ObsParams P, int4 *hdr
     }
 }
 
-#ifndef OBS_MIN_CTAS
-#define OBS_MIN_CTAS 8
+#ifndef OBS_WARPS_PER_SM
+#define OBS_WARPS_PER_SM 32          // resident render warps per SM the register budget is sized for: 64 per thread
 #endif
+// agents per tile (= warps per CTA) of the narrow and the wide render tile; TA * sizeof(T) % 16 == 0 keeps every
+// tile's byte range 16-byte aligned, and the wide tile is 32 bytes per record element
+template <typename T> constexpr int obs_tile_narrow() { return 16 / (int)sizeof(T); }
+template <typename T> constexpr int obs_tile_wide() { return 32 / (int)sizeof(T); }
 #ifndef OBS_CHUNK
 #define OBS_CHUNK 4                  // consecutive tiles a CTA renders before it jumps ahead by grid * OBS_CHUNK tiles
 #endif
 // NIT = view cells per lane held in registers (NIT * 32 >= in-range cells of the view whenever that is <= 256;
 // larger views take the unpipelined tail loop).
+//
+// The small-view instantiation (NIT = 4, no headings) is launched only for views of at most 4 * 32 in-range cells
+// (launch_obs_dispatch, checked again in launch_obs_typed), so it keeps its whole LUT slice in registers and carries
+// no tail loop at all: the dead tail alone cost it 84 bytes of spills per thread on sm_90a.
+template <int NIT, bool TURN> constexpr bool obs_all_cells_in_regs() { return NIT <= 4 && !TURN; }
 //
 // The tile buffer is PERSISTENT: consecutive tiles of a CTA belong to the same arena (blocked tile assignment), so
 // the zeros and the arena's minimap channels already in the buffer are still right for the next tile.  After the
@@ -991,11 +999,11 @@ __global__ void __launch_bounds__(256) obs_headers_kernel(ObsParams P, int4 *hdr
 // remembered in one packed register) and restores the self-marker cell, then marks the new observer's cells.  A
 // warp rebuilds its record (zero fill + minimap rows from L2) only when its observer's arena changes -- once or
 // twice per launch.
-template <typename T, int NIT, bool TURN>
-__global__ void __launch_bounds__(32 * ObsOut<T>::TA, OBS_MIN_CTAS * OBS_TA_N / ObsOut<T>::TA)
+template <typename T, int NIT, bool TURN, int TA>
+__global__ void __launch_bounds__(32 * TA, OBS_WARPS_PER_SM / TA)
 obs_render_kernel(const __grid_constant__ ObsParams P) {
     const int n_total = min(P.n_total, __ldg(P.off + P.A));   // the host may hold pre-cull counts (upper bounds)
-    constexpr int OBS_TA = ObsOut<T>::TA;
+    constexpr int OBS_TA = TA;
     constexpr int OBS_THREADS = 32 * OBS_TA;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     T *buf = (T *)smem_raw;                                   // one tile: OBS_TA records
@@ -1040,30 +1048,42 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
     const int n_in = n_in_s;
     const int n_tiles = (n_total + OBS_TA - 1) / OBS_TA;
     // this lane's slice of the view LUT never changes: small views keep it in registers, large ones re-read smem
-    constexpr bool LUT_REGS = NIT <= 4 && !TURN;
+    constexpr bool LUT_REGS = obs_all_cells_in_regs<NIT, TURN>();
     int2 lreg[LUT_REGS ? NIT : 1];
     if (LUT_REGS) {
 #pragma unroll
-        for (int it = 0; it < (LUT_REGS ? NIT : 1); ++it) lreg[it] = it * 32 + lane < n_in ? lut[it * 32 + lane] : make_int2(-1, 0);
+        for (int it = 0; it < (LUT_REGS ? NIT : 1); ++it) lreg[it] = it * 32 + lane < n_in ? lut[it * 32 + lane] : make_int2(0, 0);
     }
     // hd = heading of the observer (always 0 without turn_mode)
     auto lutv = [&](int it, int hd) -> int2 {
-        if (TURN) return it * 32 + lane < n_in ? lut[hd * lut_stride + it * 32 + lane] : make_int2(-1, 0);
-        return LUT_REGS ? lreg[LUT_REGS ? it : 0] : (it * 32 + lane < n_in ? lut[it * 32 + lane] : make_int2(-1, 0));
+        if (TURN) return it * 32 + lane < n_in ? lut[hd * lut_stride + it * 32 + lane] : make_int2(0, 0);
+        return LUT_REGS ? lreg[LUT_REGS ? it : 0] : (it * 32 + lane < n_in ? lut[it * 32 + lane] : make_int2(0, 0));
     };
     // position of an observer's own cell in the padded planes (header word h = {x, y, arena, self cell | heading << 16})
     auto plane_base = [&](const int4 &h) -> long { return h.z * P.kplane + (long)(h.y + P.kpad) * P.kw + h.x + P.kpad; };
 
-    // issue the kind-plane loads of one observer; the pad makes every view cell addressable
-    auto load_kinds = [&](const int4 &h, bool on, int (&kd)[NIT]) {
+    // issue the kind-plane loads of one observer; the pad makes every view cell addressable.  Kinds are bytes: cell
+    // `it` of a lane is byte it & 3 of kd[it >> 2].  The loads are unconditional (lanes past n_in read the observer's
+    // own cell) and masked afterwards: per-cell predicates held across the tile loop were spilled on sm_90a.
+    constexpr int KW = (NIT + 3) / 4;
+    unsigned kmask[KW];                        // 0xff in the bytes of in-range cells
+#pragma unroll
+    for (int q = 0; q < KW; ++q) {
+        kmask[q] = 0u;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) if ((4 * q + b) * 32 + lane < n_in) kmask[q] |= 0xffu << (8 * b);
+    }
+    auto load_kinds = [&](const int4 &h, bool on, unsigned (&kd)[KW]) {
         const unsigned char *kp = P.kind_plane + plane_base(h);
         const int hd = TURN ? (h.w >> 16) & 3 : 0;
 #pragma unroll
-        for (int it = 0; it < NIT; ++it) {
-            const int2 l = lutv(it, hd);
-            kd[it] = (on && l.x >= 0 && !(OBS_ABLATE & 1)) ? __ldg(kp + l.y) : 0;
-        }
+        for (int q = 0; q < KW; ++q) kd[q] = 0u;
+#pragma unroll
+        for (int it = 0; it < NIT; ++it) kd[it >> 2] |= (unsigned)__ldg(kp + lutv(it, hd).y) << ((it & 3) * 8);
+#pragma unroll
+        for (int q = 0; q < KW; ++q) kd[q] &= (on && !(OBS_ABLATE & 1)) ? kmask[q] : 0u;
     };
+    auto kind_at = [](const unsigned (&kd)[KW], int it) -> int { return (kd[it >> 2] >> ((it & 3) * 8)) & 0xff; };
     // write (on = true) or erase what an occupied view cell shows: wall / food flag, or a group's {1, hp / max_hp}
     // channel of every kind, one byte each in two registers (byte k of chpack = channel of group k): no constant-bank
     // lookup and no branch ladder per marked cell
@@ -1079,8 +1099,9 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
 
     // tile assignment: chunks of OBS_CHUNK consecutive tiles, dealt round-robin over the CTAs.  Inside a chunk the
     // arena (almost) never changes, so the persistent tile needs no rebuild; across the grid all CTAs write inside one
-    // window of grid * OBS_CHUNK tiles (~90 MB), which keeps the output stream inside the TLB reach (blocked
-    // assignment -- one 4 MB region per CTA -- measured 20 % slower) and the planes of ~20 arenas L2-hot.
+    // window of grid * OBS_CHUNK tiles (~80 MB on H100), which keeps the output stream inside the TLB reach (a
+    // blocked assignment -- one contiguous region per CTA -- would spread it over the whole output) and the planes of
+    // ~20 arenas L2-hot.
     // Software pipeline: while tile i is composed, the kind loads of tile i+1 and the header load of tile i+2 fly.
     const int chunk = P.chunk;                 // 1 when there are too few tiles to keep every CTA busy with longer chunks
     const int chunk_jump = ((int)gridDim.x - 1) * chunk;
@@ -1090,14 +1111,14 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
     const int tile_end = n_tiles;
     const int4 zero4 = make_int4(0, 0, 0, 0);
     int4 hA = zero4, hA1 = zero4;             // headers of tile i and i+1
-    int kind[NIT];
+    unsigned kind[KW];
     // what this warp's record currently shows: the arena whose minimap rows it holds (-1: garbage), the previous
     // observer's heading, marked kinds (packed bytes; > 4 * 32 cells per lane never happens with NIT <= 8) and
     // self-marker cell with its unmarked minimap value per group lane
     int rec_arena = -1, prev_hd = 0, prev_self = -1;
-    unsigned prev_kinds[(NIT + 3) / 4];
+    unsigned prev_kinds[KW];
 #pragma unroll
-    for (int q = 0; q < (NIT + 3) / 4; ++q) prev_kinds[q] = 0u;
+    for (int q = 0; q < KW; ++q) prev_kinds[q] = 0u;
     float self_orig = 0.0f;
     bool prev_tail = false;                    // the previous observer had cells beyond NIT * 32 marked (large views)
     {
@@ -1118,11 +1139,12 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
         float thp[NIT];
 #pragma unroll
         for (int it = 0; it < NIT; ++it) {
+            const int t = kind_at(kind, it);
             thp[it] = 0.0f;
-            if (kind_is_agent(kind[it])) thp[it] = (kind[it] & KIND_FULL) ? 1.0f : __ldg(hpnp + lutv(it, hd).y);   // full hp: no load
+            if (kind_is_agent(t)) thp[it] = (t & KIND_FULL) ? 1.0f : __ldg(hpnp + lutv(it, hd).y);   // full hp: no load
         }
         // next tile's kinds, next-next tile's header
-        int kind1[NIT];
+        unsigned kind1[KW];
         const long o1 = (long)tile1 * OBS_TA + warp;
         load_kinds(hA1, o1 < n_total, kind1);
         int4 hA2 = zero4;
@@ -1167,10 +1189,10 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
                 // undo the previous observer: its marked cells and its self marker
 #pragma unroll
                 for (int it = 0; it < NIT; ++it) {
-                    const int t = (prev_kinds[it >> 2] >> ((it & 3) * 8)) & 0xff;
+                    const int t = kind_at(prev_kinds, it);
                     if (t != 0) mark(dst + lutv(it, prev_hd).x, t, 0.0f, false);
                 }
-                if (prev_tail) {                                                   // large views: recompute which tail cells were marked
+                if (!LUT_REGS && prev_tail) {                                                   // large views: recompute which tail cells were marked
                     for (int k = NIT * 32 + lane; k < n_in; k += 32) {
                         T *px = dst + lut[(TURN ? prev_hd * lut_stride : 0) + k].x;
                         for (int ch = 0; ch < P.C; ++ch) {
@@ -1192,16 +1214,15 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
             prev_self = self;
             prev_hd = hd;
 #pragma unroll
-            for (int q = 0; q < (NIT + 3) / 4; ++q) prev_kinds[q] = 0u;
-#pragma unroll
             for (int it = 0; it < NIT; ++it) {
-                const int t = kind[it];
-                prev_kinds[it >> 2] |= (unsigned)t << ((it & 3) * 8);
+                const int t = kind_at(kind, it);
                 if (t != 0) mark(dst + lutv(it, hd).x, t, thp[it], true);
             }
+#pragma unroll
+            for (int q = 0; q < KW; ++q) prev_kinds[q] = kind[q];
             prev_tail = false;
             const unsigned char *kindp = P.kind_plane + plane_base(hA);
-            for (int k = NIT * 32 + lane; k < n_in; k += 32) {                          // views with > NIT * 32 in-range cells
+            for (int k = NIT * 32 + lane; !LUT_REGS && k < n_in; k += 32) {                          // views with > NIT * 32 in-range cells
                 const int2 l = lut[(TURN ? hd * lut_stride : 0) + k];
                 const int t = __ldg(kindp + l.y);
                 if (t != 0) { mark(dst + l.x, t, kind_is_agent(t) ? ((t & KIND_FULL) ? 1.0f : __ldg(hpnp + l.y)) : 0.0f, true); }
@@ -1226,21 +1247,47 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
         // rotate the pipeline
         hA = hA1; hA1 = hA2;
 #pragma unroll
-        for (int it = 0; it < NIT; ++it) kind[it] = kind1[it];
+        for (int q = 0; q < KW; ++q) kind[q] = kind1[q];
     }
     if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
-template <typename T, int NIT, bool TURN>
-static void launch_obs_typed(Ctx *c, int cfg_slot, const EngineDev &hE, ObsParams &P, int n_total,
-                             bool with_headers = true, bool headers_only = false) {
+// CTAs per SM of one render instantiation at this shared-memory size (0: it does not fit), cached per context slot
+template <typename T, int NIT, bool TURN, int TA>
+static int obs_ctas_per_sm(Ctx *c, int cfg_slot, size_t smem) {
+    if (smem > 227 * 1024) return 0;
+    Ctx::ObsCfg &cfg = c->obs_cfg[cfg_slot];
+    ensure_dynamic_smem(c->device, ATTR_OBS0 + cfg_slot, obs_render_kernel<T, NIT, TURN, TA>, smem);
+    if (smem != cfg.smem) {
+        CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cfg.ctas_per_sm, obs_render_kernel<T, NIT, TURN, TA>, 32 * TA, smem));
+        cfg.smem = smem;
+    }
+    return cfg.ctas_per_sm;
+}
+
+template <typename T, int NIT, bool TURN, int TA>
+static void launch_obs_render(Ctx *c, ObsParams &P, int n_total, size_t smem, int ctas_per_sm) {
     const int g_sms = c->sms;
-    constexpr int TA = ObsOut<T>::TA;
-    constexpr int THREADS = 32 * TA;
-    const size_t tile_bytes = (size_t)TA * P.rec * sizeof(T);            // multiple of 16 by construction of TA
-    const size_t smem = tile_bytes + (size_t)(P.turn ? 4 : 1) * ((P.cells + 1) & ~1) * sizeof(int2);
-    if (smem > 227 * 1024) mg::fatal("observation record too large for the render kernel (%zu bytes of shared memory)", smem);
     const int tiles = (n_total + TA - 1) / TA;
+    const int grid = tiles < ctas_per_sm * g_sms ? tiles : ctas_per_sm * g_sms;
+    P.chunk = tiles / (ctas_per_sm * g_sms);                            // keep every CTA busy before lengthening chunks
+    if (P.chunk < 1) P.chunk = 1;
+    const int max_chunk = sizeof(T) == 2 ? 2 * OBS_CHUNK : OBS_CHUNK;   // f16 tiles are rebuilt for twice the observers at once: longer chunks pay
+    if (P.chunk > max_chunk) P.chunk = max_chunk;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    const bool timed = c->profile && !c->capturing;
+    if (timed) { profile_pair(c, &e0, &e1); CUDA_CHECK(cudaEventRecord(e0, c->stream)); }
+    obs_render_kernel<T, NIT, TURN, TA><<<grid, 32 * TA, smem, c->stream>>>(P);
+    post_launch("obs_render_kernel");
+    if (timed) CUDA_CHECK(cudaEventRecord(e1, c->stream));
+}
+
+// cfg_slot: 0..5, one per (T, NIT, TURN); each owns two context slots, one per tile width
+template <typename T, int NIT, bool TURN>
+static void launch_obs_typed(Ctx *c, int cfg_slot, const EngineDev &hE, ObsParams &P, int n_total, int view_count,
+                             bool with_headers = true, bool headers_only = false) {
+    if (obs_all_cells_in_regs<NIT, TURN>() && view_count > NIT * 32)
+        mg::fatal("render kernel NIT=%d chosen for a view of %d in-range cells", NIT, view_count);
     if ((size_t)n_total > c->obs_hdr_n) {                                // scratch owned by the context: per-agent headers
         no_capture(c, "growing the observation header table");
         if (c->obs_hdr) { CUDA_CHECK(cudaStreamSynchronize(c->stream)); cudaFree(c->obs_hdr); }
@@ -1258,25 +1305,16 @@ static void launch_obs_typed(Ctx *c, int cfg_slot, const EngineDev &hE, ObsParam
         post_launch("obs_headers_kernel");
     }
     if (headers_only) return;
-    Ctx::ObsCfg &cfg = c->obs_cfg[cfg_slot];
-    ensure_dynamic_smem(c->device, ATTR_OBS0 + cfg_slot, obs_render_kernel<T, NIT, TURN>, smem);
-    if (smem != cfg.smem) {
-        CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cfg.ctas_per_sm, obs_render_kernel<T, NIT, TURN>, THREADS, smem));
-        if (cfg.ctas_per_sm < 1) cfg.ctas_per_sm = 1;
-        cfg.smem = smem;
-    }
-    const int ctas_per_sm = cfg.ctas_per_sm;
-    const int grid = tiles < ctas_per_sm * g_sms ? tiles : ctas_per_sm * g_sms;
-    P.chunk = tiles / (ctas_per_sm * g_sms);                            // keep every CTA busy before lengthening chunks
-    if (P.chunk < 1) P.chunk = 1;
-    const int max_chunk = sizeof(T) == 2 ? 2 * OBS_CHUNK : OBS_CHUNK;   // f16 tiles are rebuilt for 8 observers at once: longer chunks pay (measured)
-    if (P.chunk > max_chunk) P.chunk = max_chunk;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    const bool timed = c->profile && !c->capturing;
-    if (timed) { profile_pair(c, &e0, &e1); CUDA_CHECK(cudaEventRecord(e0, c->stream)); }
-    obs_render_kernel<T, NIT, TURN><<<grid, THREADS, smem, c->stream>>>(P);
-    post_launch("obs_render_kernel");
-    if (timed) CUDA_CHECK(cudaEventRecord(e1, c->stream));
+    // the wide tile whenever it keeps at least as many warps per SM as the narrow one (always, for battle); the
+    // narrow tile for records whose wide tile fits fewer warps or not at all
+    constexpr int TN = obs_tile_narrow<T>(), TW = obs_tile_wide<T>();
+    const size_t lut_bytes = (size_t)(P.turn ? 4 : 1) * ((P.cells + 1) & ~1) * sizeof(int2);
+    const size_t smem_n = (size_t)TN * P.rec * sizeof(T) + lut_bytes, smem_w = (size_t)TW * P.rec * sizeof(T) + lut_bytes;
+    if (smem_n > 227 * 1024) mg::fatal("observation record too large for the render kernel (%zu bytes of shared memory)", smem_n);
+    const int ctas_w = obs_ctas_per_sm<T, NIT, TURN, TW>(c, 2 * cfg_slot + 1, smem_w);
+    const int ctas_n = obs_ctas_per_sm<T, NIT, TURN, TN>(c, 2 * cfg_slot, smem_n);
+    if (ctas_w >= 1 && ctas_w * TW >= ctas_n * TN) launch_obs_render<T, NIT, TURN, TW>(c, P, n_total, smem_w, ctas_w);
+    else launch_obs_render<T, NIT, TURN, TN>(c, P, n_total, smem_n, ctas_n < 1 ? 1 : ctas_n);
 }
 
 static void fill_obs_params(Ctx *c, const EngineDev &hE, const ObsArgs &O, const float *mm_val, int n_total, ObsParams &P) {
@@ -1307,16 +1345,17 @@ static void fill_obs_params(Ctx *c, const EngineDev &hE, const ObsArgs &O, const
 }
 
 static void launch_obs_dispatch(Ctx *c, const EngineDev &hE, const ObsArgs &O, ObsParams &P, int n_total, bool with_headers, bool headers_only) {
-    const bool small_view = hE.grp[O.group].view_count <= 4 * 32;   // in-range view cells held in registers: 4 or 8 per lane
+    const int vc = hE.grp[O.group].view_count;
+    const bool small_view = vc <= 4 * 32;                       // in-range view cells held in registers: 4 or 8 per lane
     if (hE.turn_mode) {                                         // headings: per-heading LUTs in shared memory (NIT = 8 code path)
-        if (O.half) launch_obs_typed<__half, 8, true>(c, 0, hE, P, n_total, with_headers, headers_only);
-        else launch_obs_typed<float, 8, true>(c, 1, hE, P, n_total, with_headers, headers_only);
+        if (O.half) launch_obs_typed<__half, 8, true>(c, 0, hE, P, n_total, vc, with_headers, headers_only);
+        else launch_obs_typed<float, 8, true>(c, 1, hE, P, n_total, vc, with_headers, headers_only);
     } else if (O.half) {
-        if (small_view) launch_obs_typed<__half, 4, false>(c, 2, hE, P, n_total, with_headers, headers_only);
-        else launch_obs_typed<__half, 8, false>(c, 3, hE, P, n_total, with_headers, headers_only);
+        if (small_view) launch_obs_typed<__half, 4, false>(c, 2, hE, P, n_total, vc, with_headers, headers_only);
+        else launch_obs_typed<__half, 8, false>(c, 3, hE, P, n_total, vc, with_headers, headers_only);
     } else {
-        if (small_view) launch_obs_typed<float, 4, false>(c, 4, hE, P, n_total, with_headers, headers_only);
-        else launch_obs_typed<float, 8, false>(c, 5, hE, P, n_total, with_headers, headers_only);
+        if (small_view) launch_obs_typed<float, 4, false>(c, 4, hE, P, n_total, vc, with_headers, headers_only);
+        else launch_obs_typed<float, 8, false>(c, 5, hE, P, n_total, vc, with_headers, headers_only);
     }
 }
 
