@@ -35,6 +35,19 @@ int magent_b200_random_actions(EnvHandle game, GroupHandle group, void *unused, 
  * nearest-even.  buffer[0] = view [n][view_h][view_w][n_channel], buffer[1] = feature [n][feature_size];
  * host or CUDA device pointers.  Halves the HBM / PCIe bytes per observation. */
 int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **buffer);
+/* global state (centralised critics): the whole map of every arena as one image, [num_arenas][H][W][C] with
+ * C = 1 + food_mode + 2 * n_group; env_get_info(game, -1, "state_space", int[3]) gives (H, W, C).  Per map cell:
+ *   channel 0                   1.0 on a wall (border walls included)
+ *   channel 1 (food_mode only)  1.0 on food
+ *   channel base + 2g           1.0 where an agent of group g stands (every cell of its body), base = 1 + food_mode
+ *   channel base + 2g + 1       that agent's hp / max_hp
+ * and 0 elsewhere.  Every value is the one a view covering the cell shows; groups are in absolute order (group 0
+ * first), not in the observer-relative order of the views, and there are no minimap channels.  Covers every arena
+ * whatever magent_b200_select_arena says.  half = 0: float32; half = 1: IEEE binary16, the float32 value rounded to
+ * nearest-even.  `buffer` is host memory or a 16-byte aligned CUDA device pointer.  With a device pointer the call
+ * needs no agent counts: it neither synchronises nor allocates once the game runs on the device, so it can be
+ * recorded into a CUDA graph. */
+int magent_b200_get_global_state(EnvHandle game, void *buffer, int half);
 /* int64 event counters since construction: agent_steps, attacks, hits, kills, starved, moves_ok,
  * moves_blocked, steps.  Returns the number written. */
 int magent_b200_get_counters(EnvHandle game, long long *out, int capacity);

@@ -64,6 +64,7 @@ EXT_SIGNATURES = {
     "magent_b200_select_arena": ([_vp, ctypes.c_int], ctypes.c_int),
     "magent_b200_random_actions": ([_vp, ctypes.c_int, _vp, ctypes.c_ulonglong], ctypes.c_int),
     "magent_b200_get_observation_f16": ([_vp, ctypes.c_int, ctypes.POINTER(_vp)], ctypes.c_int),
+    "magent_b200_get_global_state": ([_vp, _vp, ctypes.c_int], ctypes.c_int),
     "magent_b200_get_counters": ([_vp, ctypes.POINTER(ctypes.c_longlong), ctypes.c_int], ctypes.c_int),
     "magent_b200_last_error": ([], ctypes.c_char_p),
     "magent_b200_set_profiling": ([_vp, ctypes.c_int], ctypes.c_int),

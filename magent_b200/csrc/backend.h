@@ -49,6 +49,11 @@ void launch_offsets(Ctx *, const EngineDev *dE, const EngineDev &hE);
 // minimap_mode is off) plus whatever the backend wants to precompute for the render kernel
 void launch_obs_prepare(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int obs_group, float *mm_val);
 void launch_obs(Ctx *, const EngineDev *dE, const EngineDev &hE, const ObsArgs &O, const float *mm_val, int n_total);
+// whole-map state of every arena into `out` ([A][H][W][state_channels], obs_phases.h state_compose_cell): float32, or
+// IEEE half (the float32 value rounded to nearest-even) when `half`.  A device buffer, 16-byte aligned.
+// Declared weak: the CUDA backend always defines it, a test backend may leave it out (the engine then refuses
+// magent_b200_get_global_state instead of failing to load).
+__attribute__((weak)) void launch_global_state(Ctx *, const EngineDev *dE, const EngineDev &hE, void *out, int half);
 void launch_info(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int kind, int group,
                  void *buf, int n_total);
 void launch_random_actions(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group,

@@ -73,6 +73,7 @@ struct Ctx {
     int4 *obs_hdr = nullptr; size_t obs_hdr_n = 0;
     // cudaFuncSetAttribute caches (per device: a context never changes device)
     struct ObsCfg { size_t smem = (size_t)-1; int ctas_per_sm = 1; } obs_cfg[12];
+    ObsCfg state_cfg[2];                 // global_state_kernel<float>, <__half>: CTAs per SM (smem 0 once queried)
     int *pin_done = nullptr; size_t pin_done_n = 0;         // pinned read-back of EngineDev::done
     int *pin_counts = nullptr; size_t pin_counts_n = 0;     // pinned read-back of EngineDev::off (clear_dead)
     cudaEvent_t ev_counts = nullptr;
@@ -1364,6 +1365,106 @@ void launch_obs(Ctx *c, const EngineDev *, const EngineDev &hE, const ObsArgs &O
     ObsParams P;
     fill_obs_params(c, hE, O, mm_val, n_total, P);
     launch_obs_dispatch(c, hE, O, P, n_total, true, false);
+}
+
+// ------------------------------------------------------------------------------------------------
+// global state (magent_b200_get_global_state): state_compose_cell of every map cell of every arena, [A][H][W][C] in T.
+// The output is one dense stream of 16-byte vectors, each written once.  A CTA takes tiles of GS_TILE consecutive
+// output elements (16 KB of float32, 8 KB of half) and composes each tile in shared memory, one thread per map cell:
+// consecutive threads read consecutive kind bytes of a plane row, and only agent cells below max hp load their hp_norm
+// value.  Then the tile goes out with coalesced 16-byte stores; a warp's stores cover 512 contiguous bytes.  Only a
+// ragged last vector (A*H*W*C not a multiple of the vector) is stored element by element.
+//
+// Composing per cell rather than per output vector keeps the work per element to one select chain and one shared store:
+// an output vector of 4 or 8 elements straddles cells whenever C does not divide it (battle: C = 5), and composing it
+// directly costs a kind and an hp lookup per element.
+enum { GS_THREADS = 256, GS_TILE = 4096, GS_BATCH = 4 };
+struct StateParams {
+    const unsigned char *kind;       // EngineDev::kind, padded
+    const float *hpn;                // EngineDev::hpn, padded
+    int H, W, kpad, kw;
+    long kplane;
+    int C, base;                     // state_channels, state_base
+    long long n_elem;                // A*H*W*C
+    void *out;
+};
+template <typename T> constexpr int gs_vec_elems() { return 16 / (int)sizeof(T); }
+
+template <typename T>
+__global__ void __launch_bounds__(GS_THREADS) global_state_kernel(const __grid_constant__ StateParams P) {
+    constexpr int VE = gs_vec_elems<T>(), TILE_V = GS_TILE / VE;
+    __shared__ __align__(16) T s_out[GS_TILE];
+    const long long n_tiles = (P.n_elem + GS_TILE - 1) / GS_TILE, n_full = P.n_elem / VE;
+    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const long long e0 = tile * GS_TILE;
+        const int ne = (int)min((long long)GS_TILE, P.n_elem - e0);
+        const long long c0 = e0 / P.C;                            // first cell of the tile and the tile's offset inside it
+        const int r0 = (int)(e0 - c0 * P.C);
+        const int nc = (r0 + ne - 1) / P.C + 1;
+        const int row0 = (int)(c0 / P.W), x0 = (int)(c0 - (long long)row0 * P.W);      // row = a * H + y
+        for (int i0 = threadIdx.x; i0 < nc; i0 += GS_THREADS * GS_BATCH) {
+            long pc[GS_BATCH];
+            int t[GS_BATCH];
+            float hp[GS_BATCH];
+#pragma unroll
+            for (int q = 0; q < GS_BATCH; ++q) {                  // the batch's kind loads are all in flight at once
+                const int i = i0 + q * GS_THREADS;
+                const int dr = (x0 + i) / P.W, x = x0 + i - dr * P.W;
+                const int row = row0 + dr, a = row / P.H, y = row - a * P.H;
+                pc[q] = a * P.kplane + (long)(y + P.kpad) * P.kw + x + P.kpad;
+                t[q] = i < nc ? (int)__ldg(P.kind + pc[q]) : KIND_EMPTY;
+            }
+#pragma unroll
+            for (int q = 0; q < GS_BATCH; ++q) hp[q] = state_needs_hpn(t[q]) ? __ldg(P.hpn + pc[q]) : 1.0f;
+#pragma unroll
+            for (int q = 0; q < GS_BATCH; ++q) {
+                const int le = (i0 + q * GS_THREADS) * P.C - r0;  // tile element of the cell's channel 0
+                for (int ch = 0; ch < P.C; ++ch)
+                    if (le + ch >= 0 && le + ch < ne) s_out[le + ch] = ObsOut<T>::cv(state_cell_value(t[q], hp[q], ch, P.base));
+            }
+        }
+        __syncthreads();
+        const long long v0 = e0 / VE;
+        for (int lv = threadIdx.x; lv < TILE_V; lv += GS_THREADS) {
+            const long long v = v0 + lv;
+            if (v < n_full) {
+                ((uint4 *)P.out)[v] = ((const uint4 *)s_out)[lv];
+            } else if (lv * VE < ne) {                            // the ragged end of the output
+                for (int j = lv * VE; j < ne; ++j) ((T *)P.out)[e0 + j] = s_out[j];
+            }
+        }
+        __syncthreads();
+    }
+}
+
+template <typename T>
+static void launch_global_state_typed(Ctx *c, const StateParams &P, int slot) {
+    Ctx::ObsCfg &cfg = c->state_cfg[slot];
+    if (cfg.smem != 0) {
+        CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cfg.ctas_per_sm, global_state_kernel<T>, GS_THREADS, 0));
+        if (cfg.ctas_per_sm < 1) mg::fatal("global_state_kernel does not fit an SM");
+        cfg.smem = 0;
+    }
+    const long long tiles = (P.n_elem + GS_TILE - 1) / GS_TILE;
+    const long long resident = (long long)cfg.ctas_per_sm * c->sms;
+    const unsigned grid = (unsigned)(tiles < resident ? tiles : resident);
+    if (grid == 0) return;
+    global_state_kernel<T><<<grid, GS_THREADS, 0, c->stream>>>(P);
+    post_launch("global_state_kernel");
+}
+
+void launch_global_state(Ctx *c, const EngineDev *, const EngineDev &hE, void *out, int half) {
+    DeviceGuard guard(c);
+    if ((uintptr_t)out & 15) mg::fatal("the global state buffer must be 16-byte aligned (got %p)", out);
+    StateParams P;
+    memset(&P, 0, sizeof P);
+    P.kind = hE.kind; P.hpn = hE.hpn;
+    P.H = hE.H; P.W = hE.W; P.kpad = hE.kpad; P.kw = hE.kw; P.kplane = hE.kplane;
+    P.C = state_channels(hE); P.base = state_base(hE);
+    P.n_elem = (long long)hE.A * hE.H * hE.W * P.C;
+    P.out = out;
+    if (half) launch_global_state_typed<__half>(c, P, 1);
+    else launch_global_state_typed<float>(c, P, 0);
 }
 
 // ------------------------------------------------------------------------------------------------

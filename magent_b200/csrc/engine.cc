@@ -987,6 +987,20 @@ void Engine::get_observation_wire(int group, void **bufs) {
     io_[IO_HOST_WRITTEN] += (long long)n * g.rec * 4 + (fpinned ? 0 : (long long)fbytes);
 }
 
+// The global state has a fixed shape, so it needs no agent counts: a device buffer takes one kernel and no host
+// synchronisation (recordable into a graph).  It always covers every arena, whatever select_arena says, and leaves the
+// observation pre-pass cache alone.  A host buffer goes through the device staging the dense observations use.
+void Engine::get_global_state(void *buf, int half) {
+    if (!be::launch_global_state) fatal("the %s backend has no global-state kernel", be::name());
+    to_device();
+    if (be::is_device_ptr(buf)) { be::launch_global_state(bx_, dE_, hE_, buf, half ? 1 : 0); return; }
+    const size_t bytes = (size_t)A_ * H_ * W_ * state_channels() * (half ? 2 : 4);
+    stage_reserve(d_view_stage_, view_stage_bytes_, bytes);
+    be::launch_global_state(bx_, dE_, hE_, d_view_stage_, half ? 1 : 0);
+    be::d2h(bx_, buf, d_view_stage_, bytes);
+    io_[IO_D2H] += (long long)bytes;
+}
+
 void Engine::set_action(int group, const int *actions) {              // GridWorld.cc:403-454
     check_group(group, "GridWorld::set_action");
     to_device();
@@ -1257,8 +1271,12 @@ int Engine::get_counters(long long *out, int cap) {
 }
 
 void Engine::get_info(int group, const char *name, void *void_buffer) {        // GridWorld.cc:709-894
-    settle_counts();
     int *ib = (int *)void_buffer;
+    if (strequ(name, "state_space")) {                  // extension: per-arena shape of magent_b200_get_global_state
+        ib[0] = H_; ib[1] = W_; ib[2] = state_channels();               // fixed: no counts needed, nothing to wait for
+        return;
+    }
+    settle_counts();
     float *fb = (float *)void_buffer;
     if (strequ(name, "num")) {
         check_group(group, "get_info(num)");

@@ -96,6 +96,8 @@ public:
     // ---- extensions
     void select_arena(int a) { sel_arena_ = a; }
     void random_actions(int group, unsigned long long seed);
+    // whole-map state of every arena, [A][H][W][state_channels()] (obs_phases.h state_compose_cell); half: IEEE binary16
+    void get_global_state(void *buf, int half);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads
@@ -167,6 +169,7 @@ private:
     int G() const { return (int)group_type_.size(); }
     int group2channel(int g) const;
     int n_channel() const { return group2channel(G()); }
+    int state_channels() const { return 1 + (food_mode_ ? 1 : 0) + 2 * G(); }     // = mg::state_channels(hE_)
     int feature_size(int g) const;
     int total(int g) const { return h_off_[(size_t)g * (A_ + 1) + A_]; }
     int count(int g, int a) const { return h_off_[(size_t)g * (A_ + 1) + a + 1] - h_off_[(size_t)g * (A_ + 1) + a]; }

@@ -63,6 +63,31 @@ MG_HD void obs_compose_cell(const EngineDev &E, unsigned curmask, int a, int g, 
     out[ch + 1] = (E.kind[pc] & KIND_FULL) ? 1.0f : E.hpn[pc];
 }
 
+// ---- global state (magent_b200_get_global_state): the whole map of every arena, [A][H][W][state_channels] floats.
+// Channel 0 is the wall, 1 the food (food_mode only), then per group g in ABSOLUTE order base + 2g is presence and
+// base + 2g + 1 the occupant's hp / max_hp.  Every value equals what Map::extract_view (Map.cc:191-199) writes for that map
+// cell into any view covering it; only the channel order differs from a view's observer-relative one (obs_channel).
+MG_HD int state_base(const EngineDev &E) { return 1 + (E.food_mode ? 1 : 0); }
+MG_HD int state_channels(const EngineDev &E) { return state_base(E) + 2 * E.G; }
+// the cell's hp / max_hp lives in the hp_norm plane: an agent below max_hp (KIND_FULL agents show 1.0f)
+MG_HD bool state_needs_hpn(int t) { return kind_is_agent(t) && !(t & KIND_FULL); }
+// channel ch of a cell whose kind byte is t; hp is the hp / max_hp the cell shows when it holds an agent
+MG_HD float state_cell_value(int t, float hp, int ch, int base) {
+    if (t == KIND_EMPTY) return 0.0f;
+    if (t == KIND_WALL) return ch == 0 ? 1.0f : 0.0f;
+    if (t == KIND_FOOD) return ch == 1 ? 1.0f : 0.0f;
+    const int c = base + 2 * kind_group(t);
+    return ch == c ? 1.0f : ch == c + 1 ? hp : 0.0f;
+}
+// the state_channels floats of map cell (x, y) of arena a, read from the padded planes the render reads
+MG_HD void state_compose_cell(const EngineDev &E, int a, int x, int y, float *out) {
+    const long pc = a * E.kplane + (long)(y + E.kpad) * E.kw + x + E.kpad;
+    const int t = E.kind[pc];
+    const float hp = state_needs_hpn(t) ? E.hpn[pc] : 1.0f;
+    const int base = state_base(E), C = state_channels(E);
+    for (int ch = 0; ch < C; ++ch) out[ch] = state_cell_value(t, hp, ch, base);
+}
+
 // non-spatial feature vector of agent (a, g, i)  (GridWorld.cc:386-396, Agent::get_embedding GridWorld.h:155-164)
 MG_HD void obs_feature(const EngineDev &E, unsigned curmask, int a, int g, int i, float *out) {
     const GroupDev &G = E.grp[g];

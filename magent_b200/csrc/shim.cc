@@ -105,6 +105,10 @@ MG_API int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, vo
     E(game)->get_observation(group, buffer, 1);
     return 0;
 }
+MG_API int magent_b200_get_global_state(EnvHandle game, void *buffer, int half) {
+    E(game)->get_global_state(buffer, half);
+    return 0;
+}
 MG_API int magent_b200_get_counters(EnvHandle game, long long *out, int capacity) { return E(game)->get_counters(out, capacity); }
 MG_API long long magent_b200_launch_count(void) { return mg::be::launch_count(); }
 MG_API int magent_b200_set_profiling(EnvHandle game, int on) { E(game)->set_profiling(on != 0); return 0; }

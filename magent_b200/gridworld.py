@@ -453,6 +453,48 @@ class GridWorld(Environment):
         self._lib.magent_b200_get_observation_f16(self.game, g, bufs)
         return view, feat
 
+    def get_state_space(self):
+        """(H, W, C) of one arena's global state (extension; see get_global_state)"""
+        buf = np.empty((3,), dtype=np.int32)
+        self._lib.env_get_info(self.game, -1, b"state_space", buf.ctypes.data)
+        return int(buf[0]), int(buf[1]), int(buf[2])
+
+    def get_global_state(self):
+        """whole-map global state of every arena (extension): float32 (num_arenas, H, W, C).
+
+        Per map cell: channel 0 wall, channel 1 food (food_mode only), then per group g in absolute order
+        base + 2g presence and base + 2g + 1 hp / max_hp (base = 1 + food_mode); 0 elsewhere.  Every value equals
+        the one a view covering the cell shows.  The array is a cached receive buffer: valid until the next call."""
+        buf = self._get_state_buf((self.num_arenas,) + self.get_state_space())
+        self._lib.magent_b200_get_global_state(self.game, buf.ctypes.data, 0)
+        return buf
+
+    def _get_state_buf(self, shape):
+        block = self._blocks.get("state")
+        if block is None:
+            block = self._blocks["state"] = _HostBlock(self._lib)
+        return block.view(shape, np.float32)
+
+    def get_global_state_torch(self, out=None, dtype=None):
+        """the global state (see get_global_state) written straight into a CUDA tensor (num_arenas, H, W, C).
+
+        dtype: torch.float32 (default) or torch.float16 (every element the float32 value rounded to nearest-even).
+        out: a caller-owned contiguous CUDA tensor of that shape, 16-byte aligned; needed to record the call into a
+        CUDA graph (capture_graph), since the call then allocates nothing."""
+        import torch
+        shape = (self.num_arenas,) + self.get_state_space()
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float32 if dtype is None else dtype, device="cuda")
+        elif dtype is not None and out.dtype != dtype:
+            raise ValueError("out has dtype %s, not %s" % (out.dtype, dtype))
+        if out.dtype not in (torch.float32, torch.float16):
+            raise ValueError("global state dtype must be torch.float32 or torch.float16")
+        if (not out.is_cuda or tuple(out.shape) != shape or not out.is_contiguous() or out.data_ptr() % 16):
+            raise ValueError("out must be a contiguous, 16-byte aligned CUDA tensor of shape %s" % (shape,))
+        self._lib.magent_b200_get_global_state(self.game, ctypes.c_void_p(out.data_ptr()),
+                                               1 if out.dtype == torch.float16 else 0)
+        return out
+
     def set_random_actions(self, handle, seed):
         """uniform random actions generated on the device (throughput runs only)"""
         self._lib.magent_b200_random_actions(self.game, self._hv(handle), None, int(seed))
