@@ -48,6 +48,35 @@ int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **bu
  * needs no agent counts: it neither synchronises nor allocates once the game runs on the device, so it can be
  * recorded into a CUDA graph. */
 int magent_b200_get_global_state(EnvHandle game, void *buffer, int half);
+/* reset pool: restart finished arenas of the batch without leaving the device.  Take a snapshot once, after placement
+ * (placement itself stays on the host, bit-exact with the reference), and later restore any subset of arenas from it.
+ * The calls below return -1 and set magent_b200_last_error when they refuse; the state is then unchanged.
+ *
+ * snapshot_arenas copies the current state of every arena into new device memory of its own and returns the
+ * snapshot's id (>= 0).  Ids are not reused; free_snapshot releases one.  A snapshot restored inside a recorded CUDA
+ * graph lives as long as the game. */
+int magent_b200_snapshot_arenas(EnvHandle game);
+int magent_b200_free_snapshot(EnvHandle game, int snapshot);
+/* src: int32[num_arenas], host or CUDA device pointer.  src[a] = -1 keeps arena a byte for byte; src[a] = s in
+ * [0, num_arenas) makes it exactly arena s of the snapshot: map, food, every agent with its order, ids, hp, rewards,
+ * last op and heading, the per-arena counters and reward state, the done flag, the agent id counter, and, when
+ * keep_rng = 0, the RNG state (keep_rng = 1: the arena keeps its own minstd stream).  src == NULL: every arena whose
+ * last env_step reported done is replaced by its own index (src[a] = a), decided on the device.  On the device,
+ * values outside [0, num_arenas) mean -1; a host src holding one is refused.  magent_b200_select_arena does not apply.
+ * Refused: actions set for the current step (call env_step first), rendering started, an unknown or freed snapshot,
+ * a snapshot taken under another geometry (map size, groups, agent types, food_mode, turn_mode).
+ * With a device pointer or NULL the call neither synchronises nor allocates, so it can be recorded into a CUDA graph.
+ *
+ * Counts: env_get_info "num" stays exact (it waits for the counts, as after gridworld_clear_dead).  Without waiting,
+ * env_get_info(game, -1, "num_bound", int[n_group]) gives per group the most records a device-pointer call can write
+ * before the counts next settle.  While any snapshot exists, a CUDA graph sizes every count-dependent launch it records
+ * (before or after a restore) for the counts a restore can produce: size the device buffers of such a graph by
+ * "num_bound".  env_get_info(game, -1, "arena_rng", uint32[num_arenas]) gives each arena's minstd state (a value for
+ * the "seed" key would have to be this to continue the stream). */
+int magent_b200_restore_arenas(EnvHandle game, int snapshot, const int *src, int keep_rng);
+/* per-arena done flags of the last env_step into int32[num_arenas], host or CUDA device pointer; with a device pointer
+ * nothing is waited for */
+int magent_b200_get_arena_done(EnvHandle game, int *out);
 /* int64 event counters since construction: agent_steps, attacks, hits, kills, starved, moves_ok,
  * moves_blocked, steps.  Returns the number written. */
 int magent_b200_get_counters(EnvHandle game, long long *out, int capacity);

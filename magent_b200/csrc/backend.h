@@ -54,6 +54,16 @@ void launch_obs(Ctx *, const EngineDev *dE, const EngineDev &hE, const ObsArgs &
 // Declared weak: the CUDA backend always defines it, a test backend may leave it out (the engine then refuses
 // magent_b200_get_global_state instead of failing to load).
 __attribute__((weak)) void launch_global_state(Ctx *, const EngineDev *dE, const EngineDev &hE, void *out, int half);
+// Restore arenas from a snapshot (Engine::restore_arenas): live arena a becomes snapshot arena s = src[a] (src: device
+// int32[A]), or s = a where bit 0 of EngineDev::done[a] is set when src is nullptr; s outside [0, A) leaves the arena
+// untouched.  Copies occ, kind, hp_norm, food, the first S.n[g][s] records of every SoA field of the live buffer
+// (curmask), n, dead_ct, done and the header (but the RNG when keep_rng), fills claim_head with -1, then recomputes the
+// offset table (launch_offsets).  Needs no host synchronisation.
+// launch_arena_done: bit 0 of EngineDev::done into out[A] (a device buffer).
+// Declared weak like launch_global_state: a backend without them loads, and the engine refuses the calls.
+__attribute__((weak)) void launch_restore(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask,
+                                          const SnapDev &S, const int *src, int keep_rng);
+__attribute__((weak)) void launch_arena_done(Ctx *, const EngineDev *dE, const EngineDev &hE, int *out);
 void launch_info(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int kind, int group,
                  void *buf, int n_total);
 void launch_random_actions(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group,

@@ -74,6 +74,7 @@ struct Ctx {
     // cudaFuncSetAttribute caches (per device: a context never changes device)
     struct ObsCfg { size_t smem = (size_t)-1; int ctas_per_sm = 1; } obs_cfg[12];
     ObsCfg state_cfg[2];                 // global_state_kernel<float>, <__half>: CTAs per SM (smem 0 once queried)
+    int restore_ctas_per_sm = 0;         // restore_kernel (0: not queried yet)
     int *pin_done = nullptr; size_t pin_done_n = 0;         // pinned read-back of EngineDev::done
     int *pin_counts = nullptr; size_t pin_counts_n = 0;     // pinned read-back of EngineDev::off (clear_dead)
     cudaEvent_t ev_counts = nullptr;
@@ -623,9 +624,8 @@ void launch_cull(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curm
     }
 }
 
-// off[g][0..A] = exclusive prefix of n[g][0..A-1]; one CTA per group
-__global__ void __launch_bounds__(1024) offsets_kernel(const EngineDev *gE) {
-    const int g = blockIdx.x;
+// off[g][0..A] = exclusive prefix of n[g][0..A-1], by one whole CTA
+__device__ __forceinline__ void offsets_group(const EngineDev *gE, int g) {
     const int A = gE->A;
     const int *n = gE->n + (size_t)g * A;
     int *off = gE->off + (size_t)g * (A + 1);
@@ -640,6 +640,9 @@ __global__ void __launch_bounds__(1024) offsets_kernel(const EngineDev *gE) {
     }
     if (threadIdx.x == 0) off[A] = running;
 }
+
+// one CTA per group
+__global__ void __launch_bounds__(1024) offsets_kernel(const EngineDev *gE) { offsets_group(gE, blockIdx.x); }
 
 void launch_offsets(Ctx *c, const EngineDev *dE, const EngineDev &hE) {
     DeviceGuard guard(c);
@@ -1465,6 +1468,168 @@ void launch_global_state(Ctx *c, const EngineDev *, const EngineDev &hE, void *o
     P.out = out;
     if (half) launch_global_state_typed<__half>(c, P, 1);
     else launch_global_state_typed<float>(c, P, 0);
+}
+
+// ------------------------------------------------------------------------------------------------
+// restore_kernel: arenas of a snapshot copied over live arenas (Engine::restore_arenas, DESIGN.md §5).
+//
+// Work items are (arena, chunk) pairs, K chunks of about RS_CHUNK_BYTES per arena, dealt grid-stride to at most one wave
+// of CTAs.  Large chunks: an item walks some 30 segments one after the other, and a thread needs several vectors of each
+// in flight (battle512 on H100: 16 KB chunks restore every arena in 1.14 ms, 512 KB chunks in 0.25 ms).  An item
+// reads its arena's source (src[a], or a itself when src is null and the arena's last step reported done) and is
+// finished at once when there is none, so a restore of nothing costs one launch of idle CTAs.  Otherwise chunk k copies
+// the k-th of K slices of every segment of the arena: the occ, kind, hp_norm and food planes, the snapshot's n[g][s]
+// records of every SoA field, and the -1 fill of claim_head.  A segment's slices are 16-byte vectors where source and
+// destination agree modulo 16 bytes (SoA capacities are multiples of 64; a plane does when its per-arena size is a
+// multiple of 16 bytes or the arena restores itself), else words or bytes; the unaligned head and the ragged tail go
+// to chunk 0.  Chunk 0 also copies counts and header.
+//
+// The done words are written by restore_finish_kernel afterwards: with a null src every chunk of an arena reads its
+// arena's done word to decide, so no chunk may change it.
+enum { RS_THREADS = 256, RS_CHUNK_BYTES = 512 << 10, RS_MAX_CHUNKS = 256, RS_SOA_FIELDS = 11, RS_SOA_WORDS = 8 };
+static_assert(sizeof(AgentSoA) == RS_SOA_FIELDS * sizeof(void *), "AgentSoA: 8 four-byte fields, then 3 byte fields");
+static_assert(offsetof(ArenaHdr, rng) == 0 && offsetof(ArenaHdr, rng_next) == 4 && sizeof(ArenaHdr) % 4 == 0,
+              "keep_rng skips the first two words of the header");
+
+struct RestoreParams {
+    const int *src;                  // device int32[A] or nullptr (done-driven)
+    const int *done;                 // EngineDev::done
+    int A, G, K, keep_rng;
+    long cells, kplane;              // W*H, padded plane
+    int *occ, *claim; unsigned char *kind; float *hpn, *food;
+    ArenaHdr *hdr; int *n, *dead_ct;
+    int cap[MG_MAX_GROUPS];
+    AgentSoA soa[MG_MAX_GROUPS];     // the live ping-pong buffer
+    SnapDev S;
+};
+
+// slice k of K of a copy in units of T; dst and src agree modulo sizeof(T)
+template <typename T>
+__device__ __forceinline__ void rs_copy_as(unsigned char *dst, const unsigned char *src, long bytes, int k, int K) {
+    constexpr long U = sizeof(T);
+    const long head = min(bytes, (long)((U - ((uintptr_t)dst & (U - 1))) & (U - 1)));
+    const long nv = (bytes - head) / U;
+    if (k == 0) {
+        for (long i = threadIdx.x; i < head; i += RS_THREADS) dst[i] = src[i];
+        for (long i = head + nv * U + threadIdx.x; i < bytes; i += RS_THREADS) dst[i] = src[i];
+    }
+    T *d = (T *)(dst + head);
+    const T *s = (const T *)(src + head);
+    const long v1 = nv * (k + 1) / K;
+#pragma unroll 4
+    for (long v = nv * k / K + threadIdx.x; v < v1; v += RS_THREADS) d[v] = __ldg(s + v);
+}
+
+// 16-byte vectors where source and destination agree modulo 16 (every SoA field, and the planes of a restore from the
+// same arena or of maps whose plane size is a multiple of 16 bytes), else words or bytes
+__device__ __forceinline__ void rs_copy(unsigned char *dst, const unsigned char *src, long bytes, int k, int K) {
+    const unsigned rel = (unsigned)((uintptr_t)dst - (uintptr_t)src) & 15u;
+    if (rel == 0) rs_copy_as<uint4>(dst, src, bytes, k, K);
+    else if ((rel & 3u) == 0) rs_copy_as<unsigned>(dst, src, bytes, k, K);
+    else rs_copy_as<unsigned char>(dst, src, bytes, k, K);
+}
+
+__device__ __forceinline__ void rs_fill_ff(unsigned char *dst, long bytes, int k, int K) {
+    const long head = min(bytes, (long)((16 - ((uintptr_t)dst & 15)) & 15));
+    const long nv = (bytes - head) >> 4;
+    if (k == 0) {
+        for (long i = threadIdx.x; i < head; i += RS_THREADS) dst[i] = 0xff;
+        for (long i = head + (nv << 4) + threadIdx.x; i < bytes; i += RS_THREADS) dst[i] = 0xff;
+    }
+    uint4 *d = (uint4 *)(dst + head);
+    const long v1 = nv * (k + 1) / K;
+    for (long v = nv * k / K + threadIdx.x; v < v1; v += RS_THREADS) d[v] = make_uint4(~0u, ~0u, ~0u, ~0u);
+}
+
+__device__ __forceinline__ int restore_source(const int *src, const int *done, int A, int a) {
+    const int s = src ? __ldg(src + a) : ((__ldg(done + a) & 1) ? a : -1);
+    return s >= 0 && s < A ? s : -1;
+}
+
+__global__ void __launch_bounds__(RS_THREADS, 4) restore_kernel(const __grid_constant__ RestoreParams P) {
+    const long items = (long)P.A * P.K;
+    for (long item = blockIdx.x; item < items; item += gridDim.x) {
+        const int a = (int)(item / P.K), k = (int)(item - (long)a * P.K);
+        const int s = restore_source(P.src, P.done, P.A, a);
+        if (s < 0) continue;
+        rs_copy((unsigned char *)(P.occ + a * P.cells), (const unsigned char *)(P.S.occ + s * P.cells), P.cells * 4, k, P.K);
+        rs_fill_ff((unsigned char *)(P.claim + a * P.cells), P.cells * 4, k, P.K);
+        rs_copy(P.kind + a * P.kplane, P.S.kind + s * P.kplane, P.kplane, k, P.K);
+        rs_copy((unsigned char *)(P.hpn + a * P.kplane), (const unsigned char *)(P.S.hpn + s * P.kplane), P.kplane * 4, k, P.K);
+        if (P.food)
+            rs_copy((unsigned char *)(P.food + a * P.cells), (const unsigned char *)(P.S.food + s * P.cells), P.cells * 4, k, P.K);
+        for (int g = 0; g < P.G; ++g) {
+            const long ns = __ldg(P.S.n + g * P.A + s);
+            unsigned char *const *dst = (unsigned char *const *)&P.soa[g];
+            const unsigned char *const *from = (const unsigned char *const *)&P.S.soa[g];
+#pragma unroll                                            // (a rolled loop keeps a stack frame and spills)
+            for (int f = 0; f < RS_SOA_FIELDS; ++f) {
+                const long esz = f < RS_SOA_WORDS ? 4 : 1;
+                rs_copy(dst[f] + (long)a * P.cap[g] * esz, from[f] + (long)s * P.S.cap[g] * esz, ns * esz, k, P.K);
+            }
+            if (k == 0 && threadIdx.x == 0) {
+                P.n[g * P.A + a] = (int)ns;
+                P.dead_ct[g * P.A + a] = __ldg(P.S.dead_ct + g * P.A + s);
+            }
+        }
+        if (k == 0) {
+            int *h = (int *)(P.hdr + a);
+            const int *hs = (const int *)(P.S.hdr + s);
+            for (int w = threadIdx.x + (P.keep_rng ? 2 : 0); w < (int)(sizeof(ArenaHdr) / 4); w += RS_THREADS) h[w] = __ldg(hs + w);
+        }
+    }
+}
+
+// the done words of the restored arenas, then the offset table (offsets_kernel's scan, every group in one CTA)
+__global__ void __launch_bounds__(1024) restore_finish_kernel(const EngineDev *gE, const int *src, const int *snap_done) {
+    const int A = gE->A;
+    for (int a = threadIdx.x; a < A; a += blockDim.x) {
+        const int s = restore_source(src, gE->done, A, a);      // this thread alone reads and writes done[a]
+        if (s >= 0) gE->done[a] = snap_done[s];
+    }
+    __syncthreads();
+    for (int g = 0; g < gE->G; ++g) offsets_group(gE, g);
+}
+
+void launch_restore(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curmask, const SnapDev &S, const int *src,
+                    int keep_rng) {
+    DeviceGuard guard(c);
+    if (c->restore_ctas_per_sm == 0) {
+        CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c->restore_ctas_per_sm, restore_kernel, RS_THREADS, 0));
+        if (c->restore_ctas_per_sm < 1) mg::fatal("restore_kernel does not fit an SM");
+    }
+    RestoreParams P;
+    memset(&P, 0, sizeof P);
+    P.src = src; P.done = hE.done;
+    P.A = hE.A; P.G = hE.G; P.keep_rng = keep_rng ? 1 : 0;
+    P.cells = (long)hE.W * hE.H; P.kplane = hE.kplane;
+    P.occ = hE.occ; P.claim = hE.claim_head; P.kind = hE.kind; P.hpn = hE.hpn; P.food = hE.food;
+    P.hdr = hE.hdr; P.n = hE.n; P.dead_ct = hE.dead_ct;
+    // chunks per arena from the bytes a restored arena moves at most (the SoA part at the snapshot's capacity)
+    long bytes = P.cells * (P.food ? 12 : 8) + P.kplane * 5;
+    for (int g = 0; g < hE.G; ++g) {
+        P.cap[g] = hE.grp[g].cap;
+        P.soa[g] = hE.grp[g].soa[(curmask >> g) & 1u];
+        bytes += (long)S.cap[g] * (4 * RS_SOA_WORDS + (RS_SOA_FIELDS - RS_SOA_WORDS));
+    }
+    const long K = (bytes + RS_CHUNK_BYTES - 1) / RS_CHUNK_BYTES;
+    P.K = (int)(K < 1 ? 1 : K > RS_MAX_CHUNKS ? RS_MAX_CHUNKS : K);
+    P.S = S;
+    const long items = (long)P.A * P.K, resident = (long)c->restore_ctas_per_sm * c->sms;
+    restore_kernel<<<(unsigned)(items < resident ? items : resident), RS_THREADS, 0, c->stream>>>(P);
+    post_launch("restore_kernel");
+    restore_finish_kernel<<<1, 1024, 0, c->stream>>>(dE, src, S.done);
+    post_launch("restore_finish_kernel");
+}
+
+__global__ void __launch_bounds__(256) arena_done_kernel(const EngineDev *gE, int *out) {
+    for (int a = blockIdx.x * blockDim.x + threadIdx.x; a < gE->A; a += gridDim.x * blockDim.x) out[a] = gE->done[a] & 1;
+}
+
+void launch_arena_done(Ctx *c, const EngineDev *dE, const EngineDev &hE, int *out) {
+    DeviceGuard guard(c);
+    arena_done_kernel<<<(hE.A + 255) / 256, 256, 0, c->stream>>>(dE, out);
+    post_launch("arena_done_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------

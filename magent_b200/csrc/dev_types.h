@@ -101,6 +101,9 @@ struct ArenaHdr {
     // group-quantified ('all' subject) event nodes, reduced once per step (phase_rule_allq): number of agents
     // violating the predicate, and min / max of the varying coordinate for in_a_line
     int allq_viol[MG_MAX_ALLQ], allq_min[MG_MAX_ALLQ], allq_max[MG_MAX_ALLQ];
+    // next agent id of the arena (HostArena::id_counter): carried here so that a restored arena's add_agents continues
+    // from the snapshot's counter.  Uploaded by to_device, read back by to_host; the step kernels never touch it.
+    int id_counter;
 };
 
 // Entity roles inside a rule.  The reference binds the rule's input symbols depth-first in order
@@ -195,6 +198,21 @@ struct EngineDev {
     int *team_scratch;                        // [2 * max CTAs] partial sums of team scans
     int *mm_count;                            // [A][G][max_view_cells] minimap histogram scratch
     int *mm_total;                            // [A][G] agents counted into the minimap
+};
+
+// A device-resident copy of every arena's state (Engine::snapshot_arenas, DESIGN.md §3): the live arena-major layout of
+// occ, kind, hp_norm and food, the headers and counts, and the live ping-pong SoA buffer of every group with the
+// snapshot's own per-group capacity `cap`.  launch_restore copies arenas of it back over live arenas.
+struct SnapDev {
+    int *occ;                                 // [A][H*W]
+    unsigned char *kind;                      // [A][kplane]
+    float *hpn;                               // [A][kplane]
+    float *food;                              // [A][H*W] (food_mode only, else nullptr)
+    ArenaHdr *hdr;                            // [A]
+    int *n, *dead_ct;                         // [G][A]
+    int *done;                                // [A]
+    int cap[MG_MAX_GROUPS];
+    AgentSoA soa[MG_MAX_GROUPS];
 };
 
 struct StepArgs {

@@ -38,6 +38,17 @@ void fatal(const char *fmt, ...) {
 
 static bool strequ(const char *a, const char *b) { return strcmp(a, b) == 0; }
 
+// a refused extension call: the message goes to magent_b200_last_error, the call returns -1 and changes nothing
+static int refuse(const char *fmt, ...) {
+    char buf[1024];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf, sizeof buf, fmt, ap);
+    va_end(ap);
+    g_last_error = buf;
+    return -1;
+}
+
 // ---------------------------------------------------------------------------------------------
 // ranges  (reference src/gridworld/Range.h:149-190; same double-precision arithmetic)
 RangeTab make_circle_range(float radius, float inner_radius, int parity) {
@@ -112,6 +123,8 @@ Engine::Engine() {
 }
 
 Engine::~Engine() {
+    for (ArenaSnapshot &sn : snaps_)
+        for (void *p : sn.allocs) be::dfree(bx_, p);
     free_device();
     if (h_feat_stage_) be::host_free(h_feat_stage_);
     if (bx_) be::destroy(bx_);
@@ -591,6 +604,18 @@ void *Engine::io_stage(size_t bytes) {
     return d_io_stage_;
 }
 
+// the padded observation planes cover the widest view window of any group, in any heading when agents can turn
+int Engine::view_pad() const {
+    int pad = 0;
+    for (int g = 0; g < G(); ++g) {
+        const AgentTypeDef &t = *group_type_[g];
+        const int ox = t.view_x_offset + t.view.x1, oy = t.view_y_offset + t.view.y1;
+        const int ext[4] = {-ox, ox + t.view.width - 1, -oy, oy + t.view.height - 1};
+        for (int e : ext) pad = std::max(pad, e + (turn_mode_ ? std::max(t.width, t.length) : 0));
+    }
+    return pad;
+}
+
 int Engine::max_agents_per_arena() const {
     int m = 0;
     for (int a = 0; a < A_; ++a) {
@@ -614,19 +639,15 @@ void Engine::to_device() {
     if (!was_reset_) fatal("environment used before reset");
     ensure_backend();
     const int Gn = G();
-    // capacities: grow-only while the geometry is unchanged
+    const int pad = view_pad();
+    // capacities: grow-only while the geometry is unchanged; they also hold every arena of every snapshot a restore
+    // may copy in
     std::vector<int> need(Gn, 0);
     for (int g = 0; g < Gn; ++g) {
         for (int a = 0; a < A_; ++a) need[g] = std::max(need[g], count(g, a));
+        for (const ArenaSnapshot &sn : snaps_)
+            if (sn.live && snap_matches(sn, pad)) need[g] = std::max(need[g], sn.max_n[g]);
         need[g] = std::max(64, (need[g] + 63) / 64 * 64);
-    }
-    // the padded observation planes cover the widest view window of any group, in any heading when agents can turn
-    int pad = 0;
-    for (int g = 0; g < Gn; ++g) {
-        const AgentTypeDef &t = *group_type_[g];
-        const int ox = t.view_x_offset + t.view.x1, oy = t.view_y_offset + t.view.y1;
-        const int ext[4] = {-ox, ox + t.view.width - 1, -oy, oy + t.view.height - 1};
-        for (int e : ext) pad = std::max(pad, e + (turn_mode_ ? std::max(t.width, t.length) : 0));
     }
     // env_config_game may change the modes between episodes (as in the reference): everything an allocation's size or
     // presence depends on is part of the predicate
@@ -821,6 +842,7 @@ void Engine::to_device() {
             memset(&hdr[a], 0, sizeof(ArenaHdr));
             hdr[a].rng = hdr[a].rng_next = arenas_[a].rng;
             hdr[a].done = done[a] = arenas_[a].done;
+            hdr[a].id_counter = arenas_[a].id_counter;
             for (int g = 0; g < Gn; ++g) {
                 hdr[a].grp_reward[g] = arenas_[a].groups[g].grp_reward;
                 hdr[a].n_cull[g] = arenas_[a].groups[g].n_cull;
@@ -884,6 +906,7 @@ void Engine::to_host(bool keep_device_authoritative) {
         }
         arenas_[a].rng = hdr[a].rng;
         arenas_[a].done = hdr[a].done;
+        arenas_[a].id_counter = hdr[a].id_counter;
     }
     if (!keep_device_authoritative) where_ = HOST;
 }
@@ -999,6 +1022,158 @@ void Engine::get_global_state(void *buf, int half) {
     be::launch_global_state(bx_, dE_, hE_, d_view_stage_, half ? 1 : 0);
     be::d2h(bx_, buf, d_view_stage_, bytes);
     io_[IO_D2H] += (long long)bytes;
+}
+
+// ---------------------------------------------------------------------------------------------
+// reset pool (DESIGN.md §3, §5): snapshots of every arena in HBM, restored into any subset of arenas by one kernel.
+// Placement stays on the host; the device only copies arena states.
+bool Engine::snap_matches(const ArenaSnapshot &s, int kpad) const {
+    return s.W == W_ && s.H == H_ && s.kpad == kpad && s.food_mode == food_mode_ && s.turn_mode == turn_mode_ &&
+           s.types == group_type_;
+}
+
+std::vector<int> Engine::restore_floor() const {
+    std::vector<int> floor(G(), 0);
+    const int pad = view_pad();
+    for (const ArenaSnapshot &sn : snaps_)
+        if (sn.live && snap_matches(sn, pad))
+            for (int g = 0; g < G(); ++g) floor[g] = std::max(floor[g], sn.max_n[g]);
+    return floor;
+}
+
+void Engine::set_counts(const std::vector<int> &c) {
+    for (int g = 0; g < G(); ++g)
+        for (int a = 0; a < A_; ++a)
+            h_off_[(size_t)g * (A_ + 1) + a + 1] = h_off_[(size_t)g * (A_ + 1) + a] + c[(size_t)g * A_ + a];
+}
+
+void Engine::raise_counts(const std::vector<int> &floor) {
+    std::vector<int> c((size_t)G() * A_);
+    for (int g = 0; g < G(); ++g)
+        for (int a = 0; a < A_; ++a) c[(size_t)g * A_ + a] = std::max(count(g, a), floor[g]);
+    set_counts(c);
+}
+
+template <class T>
+static void snap_copy(be::Ctx *bx, std::vector<void *> &allocs, T *&dst, const T *src, size_t n) {
+    dst = (T *)be::dmalloc(bx, std::max<size_t>(n, 1) * sizeof(T));
+    allocs.push_back(dst);
+    be::d2d(bx, dst, src, n * sizeof(T));
+}
+
+int Engine::snapshot_arenas() {
+    if (!was_reset_) return refuse("snapshot_arenas before reset");
+    if (bx_ && be::capturing(bx_)) return refuse("snapshot_arenas allocates device memory: not possible while a CUDA graph is being captured");
+    if (!be::launch_restore) return refuse("the %s backend has no restore kernel", be::name());
+    to_device();
+    settle_counts();
+    const int Gn = G();
+    ArenaSnapshot sn;
+    sn.live = true;
+    sn.W = W_; sn.H = H_; sn.kpad = hE_.kpad; sn.food_mode = food_mode_; sn.turn_mode = turn_mode_;
+    sn.types = group_type_;
+    sn.n.resize((size_t)Gn * A_);
+    sn.max_n.assign(Gn, 0);
+    for (int g = 0; g < Gn; ++g)
+        for (int a = 0; a < A_; ++a) {
+            sn.n[(size_t)g * A_ + a] = count(g, a);
+            sn.max_n[g] = std::max(sn.max_n[g], count(g, a));
+        }
+    SnapDev &D = sn.dev;
+    memset(&D, 0, sizeof D);
+    const size_t cells = (size_t)A_ * W_ * H_, kp = (size_t)A_ * hE_.kplane;
+    snap_copy(bx_, sn.allocs, D.occ, hE_.occ, cells);
+    snap_copy(bx_, sn.allocs, D.kind, hE_.kind, kp);
+    snap_copy(bx_, sn.allocs, D.hpn, hE_.hpn, kp);
+    if (food_mode_) snap_copy(bx_, sn.allocs, D.food, hE_.food, cells);
+    snap_copy(bx_, sn.allocs, D.hdr, hE_.hdr, (size_t)A_);
+    snap_copy(bx_, sn.allocs, D.n, hE_.n, (size_t)Gn * A_);
+    snap_copy(bx_, sn.allocs, D.dead_ct, hE_.dead_ct, (size_t)Gn * A_);
+    snap_copy(bx_, sn.allocs, D.done, hE_.done, (size_t)A_);
+    for (int g = 0; g < Gn; ++g) {                    // the live ping-pong buffer, at the live capacity
+        const AgentSoA &L = hE_.grp[g].soa[(curmask_ >> g) & 1u];
+        AgentSoA &S = D.soa[g];
+        const size_t n = (size_t)A_ * cap_[g];
+        D.cap[g] = cap_[g];
+        snap_copy(bx_, sn.allocs, S.x, L.x, n); snap_copy(bx_, sn.allocs, S.y, L.y, n);
+        snap_copy(bx_, sn.allocs, S.hp, L.hp, n); snap_copy(bx_, sn.allocs, S.act, L.act, n);
+        snap_copy(bx_, sn.allocs, S.id, L.id, n);
+        snap_copy(bx_, sn.allocs, S.next_reward, L.next_reward, n); snap_copy(bx_, sn.allocs, S.last_reward, L.last_reward, n);
+        snap_copy(bx_, sn.allocs, S.op_obj, L.op_obj, n);
+        snap_copy(bx_, sn.allocs, S.last_op, L.last_op, n); snap_copy(bx_, sn.allocs, S.flags, L.flags, n);
+        snap_copy(bx_, sn.allocs, S.dir, L.dir, n);
+    }
+    snaps_.push_back(sn);                             // ids are never reused: a freed id stays unknown
+    return (int)snaps_.size() - 1;
+}
+
+int Engine::free_snapshot(int id) {
+    if (id < 0 || id >= (int)snaps_.size() || !snaps_[id].live) return refuse("unknown or freed snapshot id %d", id);
+    ArenaSnapshot &sn = snaps_[id];
+    if (sn.in_graph) return refuse("snapshot %d is restored from inside a recorded CUDA graph: it lives as long as the game", id);
+    if (be::capturing(bx_)) return refuse("free_snapshot is not possible while a CUDA graph is being captured");
+    for (void *p : sn.allocs) be::dfree(bx_, p);
+    sn = ArenaSnapshot();
+    return 0;
+}
+
+// Counts: the host's h_off_ must stay an upper bound of the device's counts (every count-sized launch relies on it).
+// A host src gives the new counts exactly.  A device src or the done flags are only known on the device: every arena's
+// bound is raised to the snapshot's largest count and the exact counts are fetched asynchronously, as clear_dead does;
+// inside a capture they are marked unknown.
+int Engine::restore_arenas(int id, const int *src, int keep_rng) {
+    if (id < 0 || id >= (int)snaps_.size() || !snaps_[id].live) return refuse("unknown or freed snapshot id %d", id);
+    ArenaSnapshot &sn = snaps_[id];
+    if (!order_.empty()) return refuse("restore_arenas while actions are set for the current step (call env_step first)");
+    if (!first_render_) return refuse("restore_arenas while rendering is not supported");
+    if (!snap_matches(sn, view_pad()))
+        return refuse("snapshot %d was taken under a different geometry (map size, groups, agent types, food_mode or turn_mode)", id);
+    if (!be::launch_restore) return refuse("the %s backend has no restore kernel", be::name());
+    const bool capturing = bx_ && be::capturing(bx_);
+    const bool dev_src = src != nullptr && be::is_device_ptr(src);
+    if (src && !dev_src) {
+        if (capturing) return refuse("restore_arenas with a host src cannot be recorded into a CUDA graph");
+        for (int a = 0; a < A_; ++a)
+            if (src[a] < -1 || src[a] >= A_) return refuse("restore_arenas: src[%d] = %d is outside [-1, %d)", a, src[a], A_);
+    }
+    to_device();
+    const int *d_src = src;
+    if (src && !dev_src) {
+        settle_counts();
+        int *st = (int *)io_stage((size_t)A_ * 4);
+        be::h2d(bx_, st, src, (size_t)A_ * 4);
+        io_[IO_H2D] += (long long)A_ * 4;
+        d_src = st;
+    }
+    be::launch_restore(bx_, dE_, hE_, curmask_, sn.dev, d_src, keep_rng ? 1 : 0);
+    ++state_version_;
+    may_have_dead_ = true;
+    done_stale_ = true;
+    if (capturing) sn.in_graph = true;
+    if (src && !dev_src) {
+        std::vector<int> c((size_t)G() * A_);
+        for (int g = 0; g < G(); ++g)
+            for (int a = 0; a < A_; ++a) c[(size_t)g * A_ + a] = src[a] >= 0 ? sn.n[(size_t)g * A_ + src[a]] : count(g, a);
+        set_counts(c);
+        return 0;
+    }
+    raise_counts(sn.max_n);
+    if (capturing) { counts_unknown_ = true; return 0; }
+    be::counts_fetch_begin(bx_, hE_.off, h_off_.size());
+    counts_pending_ = true;
+    counts_unknown_ = false;
+    return 0;
+}
+
+int Engine::get_arena_done(int *out) {
+    if (be::is_device_ptr(out)) {
+        if (!be::launch_arena_done) return refuse("the %s backend has no arena-done kernel", be::name());
+        to_device();
+        be::launch_arena_done(bx_, dE_, hE_, out);
+        return 0;
+    }
+    get_info(-1, "arena_done", out);
+    return 0;
 }
 
 void Engine::set_action(int group, const int *actions) {              // GridWorld.cc:403-454
@@ -1242,10 +1417,16 @@ void Engine::graph_begin() {
     settle_counts();
     if (!first_render_) fatal("graph capture while rendering is not supported");
     capture_mask_ = curmask_; capture_culls_ = 0;
+    // a graph may restore arenas from any live snapshot, and a replay then starts from restored counts: while one
+    // exists, every count-sized launch of the capture, before a restore or after it, is sized for them (num_bound)
+    const std::vector<int> floor = restore_floor();
+    capture_floor_ = std::any_of(floor.begin(), floor.end(), [](int v) { return v > 0; });
+    if (capture_floor_) raise_counts(floor);
     if (!be::capture_begin(bx_)) fatal("this backend has no CUDA graph support");
 }
 int Engine::graph_end() {
     const int id = be::capture_end(bx_);
+    if (capture_floor_) { counts_unknown_ = true; capture_floor_ = false; }      // nothing ran: re-read the exact counts
     // kernel arguments are baked into the graph, the ping-pong buffer selector among them: a replay is only right when
     // the captured sequence leaves the selector where it found it (an even number of clear_dead calls)
     if (curmask_ != capture_mask_) fatal("a captured step sequence must contain an even number of clear_dead calls (got %d)", capture_culls_);
@@ -1274,6 +1455,25 @@ void Engine::get_info(int group, const char *name, void *void_buffer) {        /
     int *ib = (int *)void_buffer;
     if (strequ(name, "state_space")) {                  // extension: per-arena shape of magent_b200_get_global_state
         ib[0] = H_; ib[1] = W_; ib[2] = state_channels();               // fixed: no counts needed, nothing to wait for
+        return;
+    }
+    if (strequ(name, "num_bound")) {                    // extension: per group, records a device-pointer call may write
+        const std::vector<int> floor = restore_floor(); // before the counts next settle (no waiting here)
+        for (int g = 0; g < G(); ++g) {
+            long long n = 0;
+            for (int a = 0; a < A_; ++a) n += std::max(count(g, a), floor[g]);
+            ib[g] = (int)n;
+        }
+        return;
+    }
+    if (strequ(name, "arena_rng")) {                    // extension: uint32 minstd state of every arena
+        if (where_ == DEVICE) {
+            std::vector<ArenaHdr> hdr(A_);
+            be::d2h(bx_, hdr.data(), hE_.hdr, sizeof(ArenaHdr) * A_);
+            for (int a = 0; a < A_; ++a) ((uint32_t *)void_buffer)[a] = hdr[a].rng;
+        } else {
+            for (int a = 0; a < A_; ++a) ((uint32_t *)void_buffer)[a] = arenas_[a].rng;
+        }
         return;
     }
     settle_counts();

@@ -63,6 +63,21 @@ struct HostArena {
     int done = 0;
 };
 
+// a copy of every arena's state in HBM (Engine::snapshot_arenas): its own allocations, outside dev_allocs_, so that
+// neither free_device nor a capacity-growing re-upload frees it
+struct ArenaSnapshot {
+    bool live = false;
+    bool in_graph = false;              // recorded into a CUDA graph: lives as long as the engine
+    // the geometry it was taken under; a restore needs the same
+    int W = 0, H = 0, kpad = 0;
+    bool food_mode = false, turn_mode = false;
+    std::vector<const AgentTypeDef *> types;
+    std::vector<int> n;                 // [G][A] agents per group and arena
+    std::vector<int> max_n;             // [G] largest per-arena count
+    SnapDev dev;
+    std::vector<void *> allocs;
+};
+
 struct SymbolDef { int group = 0, index = 0; };
 struct NodeDef { int op = OP_NULL; std::vector<int> raw; };
 struct RuleDef { int on = 0; std::vector<int> recv; std::vector<float> values; bool is_terminal = false, auto_value = false; };
@@ -98,6 +113,12 @@ public:
     void random_actions(int group, unsigned long long seed);
     // whole-map state of every arena, [A][H][W][state_channels()] (obs_phases.h state_compose_cell); half: IEEE binary16
     void get_global_state(void *buf, int half);
+    // reset pool: snapshot every arena on the device, later restore any subset of arenas from it.  These return -1 and
+    // set the last error when they refuse (the state is then unchanged).
+    int snapshot_arenas();
+    int free_snapshot(int id);
+    int restore_arenas(int id, const int *src, int keep_rng);
+    int get_arena_done(int *out);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads
@@ -179,6 +200,14 @@ private:
     bool counts_pending_ = false;       // clear_dead queued a fetch of the new counts; h_off_ still holds the old (upper-bound) ones
     void settle_counts();
     void check_group(int g, const char *where) const;
+    // snapshots (reset pool)
+    std::vector<ArenaSnapshot> snaps_;
+    bool snap_matches(const ArenaSnapshot &s, int kpad) const;
+    int view_pad() const;               // kpad of the padded observation planes for the current agent types
+    std::vector<int> restore_floor() const;          // [G] largest count any usable snapshot can restore an arena to
+    void set_counts(const std::vector<int> &c);           // h_off_ from per-arena counts c[G][A]
+    void raise_counts(const std::vector<int> &floor);     // h_off_ counts to at least floor[g] in every arena
+    bool capture_floor_ = false;        // the capture in progress sizes its launches for restores (graph_begin)
 
     void ensure_backend();
     void compile_rules();

@@ -109,6 +109,12 @@ MG_API int magent_b200_get_global_state(EnvHandle game, void *buffer, int half) 
     E(game)->get_global_state(buffer, half);
     return 0;
 }
+MG_API int magent_b200_snapshot_arenas(EnvHandle game) { return E(game)->snapshot_arenas(); }
+MG_API int magent_b200_free_snapshot(EnvHandle game, int snapshot) { return E(game)->free_snapshot(snapshot); }
+MG_API int magent_b200_restore_arenas(EnvHandle game, int snapshot, const int *src, int keep_rng) {
+    return E(game)->restore_arenas(snapshot, src, keep_rng);
+}
+MG_API int magent_b200_get_arena_done(EnvHandle game, int *out) { return E(game)->get_arena_done(out); }
 MG_API int magent_b200_get_counters(EnvHandle game, long long *out, int capacity) { return E(game)->get_counters(out, capacity); }
 MG_API long long magent_b200_launch_count(void) { return mg::be::launch_count(); }
 MG_API int magent_b200_set_profiling(EnvHandle game, int on) { E(game)->set_profiling(on != 0); return 0; }

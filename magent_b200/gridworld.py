@@ -495,6 +495,66 @@ class GridWorld(Environment):
                                                1 if out.dtype == torch.float16 else 0)
         return out
 
+    # ---- reset pool: restart finished arenas from device-resident snapshots
+    def _check(self, rc, what):
+        if rc < 0:
+            raise RuntimeError("%s refused: %s" % (what, self._lib.magent_b200_last_error().decode()))
+        return rc
+
+    def snapshot_arenas(self):
+        """copy the state of every arena into a new snapshot in device memory; returns its id"""
+        return self._check(self._lib.magent_b200_snapshot_arenas(self.game), "snapshot_arenas")
+
+    def free_snapshot(self, snapshot):
+        self._check(self._lib.magent_b200_free_snapshot(self.game, int(snapshot)), "free_snapshot")
+
+    def restore_arenas(self, snapshot, src=None, keep_rng=False):
+        """make arena a exactly arena src[a] of the snapshot (src[a] = -1: leave it alone).
+
+        src: None (every arena whose last step reported done takes its own snapshot arena, decided on the device), an
+        int32 numpy array or an int32 CUDA tensor of length num_arenas (passed as a device pointer: nothing waits for the
+        host, and the call can be recorded into a CUDA graph).  keep_rng: restored arenas keep their own RNG stream."""
+        if src is None:
+            ptr = None
+        elif isinstance(src, np.ndarray):
+            if src.dtype != np.int32 or src.shape != (self.num_arenas,):
+                raise ValueError("src must be an int32 array of shape (%d,)" % self.num_arenas)
+            src = np.ascontiguousarray(src)
+            ptr = src.ctypes.data
+        else:
+            import torch
+            if (not isinstance(src, torch.Tensor) or not src.is_cuda or src.dtype != torch.int32 or
+                    tuple(src.shape) != (self.num_arenas,) or not src.is_contiguous()):
+                raise ValueError("src must be an int32 numpy array or a contiguous int32 CUDA tensor of shape (%d,)"
+                                 % self.num_arenas)
+            ptr = src.data_ptr()
+        self._check(self._lib.magent_b200_restore_arenas(self.game, int(snapshot), ptr, 1 if keep_rng else 0),
+                    "restore_arenas")
+
+    def get_arena_done_torch(self, out=None):
+        """per-arena done flags of the last step into an int32 CUDA tensor (num_arenas,); nothing waits for the host"""
+        import torch
+        if out is None:
+            out = torch.empty((self.num_arenas,), dtype=torch.int32, device="cuda")
+        if (not out.is_cuda or out.dtype != torch.int32 or tuple(out.shape) != (self.num_arenas,)
+                or not out.is_contiguous()):
+            raise ValueError("out must be a contiguous int32 CUDA tensor of shape (%d,)" % self.num_arenas)
+        self._check(self._lib.magent_b200_get_arena_done(self.game, out.data_ptr()), "get_arena_done")
+        return out
+
+    def get_arena_rng(self):
+        """uint32 minstd state of every arena (the "seed" that continues its stream)"""
+        buf = np.empty((self.num_arenas,), dtype=np.uint32)
+        self._lib.env_get_info(self.game, -1, b"arena_rng", buf.ctypes.data)
+        return buf
+
+    def get_num_bound(self, handle):
+        """the most records a device-pointer call for this group can write before the counts next settle: the size for
+        device buffers of a CUDA graph that restores arenas (see restore_arenas)"""
+        buf = np.empty((len(self.group_handles),), dtype=np.int32)
+        self._lib.env_get_info(self.game, -1, b"num_bound", buf.ctypes.data)
+        return int(buf[self._hv(handle)])
+
     def set_random_actions(self, handle, seed):
         """uniform random actions generated on the device (throughput runs only)"""
         self._lib.magent_b200_random_actions(self.game, self._hv(handle), None, int(seed))
