@@ -106,6 +106,16 @@ void *magent_b200_stream(EnvHandle game);
 int magent_b200_host_threads(void);
 int magent_b200_set_host_threads(int n);       /* 0 = default (usable cores, at most 16; 24 on hosts with 48+ usable cores) */
 
+/* ---- extension keys of the reference calls env_config_game / env_get_info (no entry point of their own) ----
+ *
+ * Render launch shape of one game (tests and measurement; the defaults are the tuned choice).  env_config_game keys,
+ * int values, changeable between calls, 0 = automatic: "obs_grid" CTAs (clamped to [1, tiles]), "obs_chunk" consecutive
+ * tiles per CTA visit (clamped to [1, ceil(tiles / grid)]), "obs_tile" 1 = narrow, 2 = wide (narrow when the wide tile
+ * does not fit in shared memory).  A negative value or obs_tile > 2 is refused: env_config_game returns -1 and nothing
+ * changes.  env_get_info(game, -1, "obs_override", int[3]) reads the three keys back.
+ * env_get_info(game, -1, "obs_launch", int[8]) reports the last obs_render_kernel launch of the game: {sizeof(T), NIT,
+ * turn, agents per tile, grid, chunk, tiles, view and feature buffers both 16-byte aligned}, zeros before the first. */
+
 #ifdef __cplusplus
 }
 #endif

@@ -49,6 +49,10 @@ void launch_offsets(Ctx *, const EngineDev *dE, const EngineDev &hE);
 // minimap_mode is off) plus whatever the backend wants to precompute for the render kernel
 void launch_obs_prepare(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int obs_group, float *mm_val);
 void launch_obs(Ctx *, const EngineDev *dE, const EngineDev &hE, const ObsArgs &O, const float *mm_val, int n_total);
+// the last obs_render_kernel launch of this context: {sizeof(T), NIT, turn, TA (agents per tile), grid, chunk, tiles,
+// view and feature buffers both 16-byte aligned}; all zero before the first launch.  Declared weak like
+// launch_global_state: a backend without it loads, and the engine refuses the "obs_launch" info key.
+__attribute__((weak)) void obs_launch_report(const Ctx *, int out[8]);
 // whole-map state of every arena into `out` ([A][H][W][state_channels], obs_phases.h state_compose_cell): float32, or
 // IEEE half (the float32 value rounded to nearest-even) when `half`.  A device buffer, 16-byte aligned.
 // Declared weak: the CUDA backend always defines it, a test backend may leave it out (the engine then refuses

@@ -17,6 +17,7 @@
 #include <stdlib.h>
 #include <string>
 #include <string.h>
+#include <algorithm>
 #include <atomic>
 #include <mutex>
 #include <vector>
@@ -73,6 +74,7 @@ struct Ctx {
     int4 *obs_hdr = nullptr; size_t obs_hdr_n = 0;
     // cudaFuncSetAttribute caches (per device: a context never changes device)
     struct ObsCfg { size_t smem = (size_t)-1; int ctas_per_sm = 1; } obs_cfg[12];
+    int obs_last[8] = {0, 0, 0, 0, 0, 0, 0, 0};            // the last render launch (obs_launch_report)
     ObsCfg state_cfg[2];                 // global_state_kernel<float>, <__half>: CTAs per SM (smem 0 once queried)
     int restore_ctas_per_sm = 0;         // restore_kernel (0: not queried yet)
     int *pin_done = nullptr; size_t pin_done_n = 0;         // pinned read-back of EngineDev::done
@@ -1269,15 +1271,25 @@ static int obs_ctas_per_sm(Ctx *c, int cfg_slot, size_t smem) {
     return cfg.ctas_per_sm;
 }
 
+// O.grid / O.chunk > 0 replace the automatic grid and chunk (tests: CTAs that render many tiles at small sizes).
+// Both are clamped: grid to [1, tiles], chunk to [1, ceil(tiles / grid)], so that the kernel's tile indices, up to
+// (grid - 1) * chunk past a tile it renders, stay far from int overflow.  The clamps never change the automatic values.
 template <typename T, int NIT, bool TURN, int TA>
-static void launch_obs_render(Ctx *c, ObsParams &P, int n_total, size_t smem, int ctas_per_sm) {
+static void launch_obs_render(Ctx *c, const ObsArgs &O, ObsParams &P, int n_total, size_t smem, int ctas_per_sm) {
     const int g_sms = c->sms;
     const int tiles = (n_total + TA - 1) / TA;
-    const int grid = tiles < ctas_per_sm * g_sms ? tiles : ctas_per_sm * g_sms;
+    int grid = tiles < ctas_per_sm * g_sms ? tiles : ctas_per_sm * g_sms;
     P.chunk = tiles / (ctas_per_sm * g_sms);                            // keep every CTA busy before lengthening chunks
     if (P.chunk < 1) P.chunk = 1;
     const int max_chunk = sizeof(T) == 2 ? 2 * OBS_CHUNK : OBS_CHUNK;   // f16 tiles are rebuilt for twice the observers at once: longer chunks pay
     if (P.chunk > max_chunk) P.chunk = max_chunk;
+    if (O.grid > 0) grid = O.grid;
+    if (O.chunk > 0) P.chunk = O.chunk;
+    grid = std::max(1, std::min(grid, tiles));
+    P.chunk = std::max(1, std::min(P.chunk, (tiles + grid - 1) / grid));
+    const int aligned = ((((size_t)P.view) | ((size_t)P.feature)) & 15) == 0;
+    const int report[8] = {(int)sizeof(T), NIT, TURN ? 1 : 0, TA, grid, P.chunk, tiles, aligned};
+    memcpy(c->obs_last, report, sizeof report);
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     const bool timed = c->profile && !c->capturing;
     if (timed) { profile_pair(c, &e0, &e1); CUDA_CHECK(cudaEventRecord(e0, c->stream)); }
@@ -1288,8 +1300,8 @@ static void launch_obs_render(Ctx *c, ObsParams &P, int n_total, size_t smem, in
 
 // cfg_slot: 0..5, one per (T, NIT, TURN); each owns two context slots, one per tile width
 template <typename T, int NIT, bool TURN>
-static void launch_obs_typed(Ctx *c, int cfg_slot, const EngineDev &hE, ObsParams &P, int n_total, int view_count,
-                             bool with_headers = true, bool headers_only = false) {
+static void launch_obs_typed(Ctx *c, int cfg_slot, const EngineDev &hE, const ObsArgs &O, ObsParams &P, int n_total,
+                             int view_count, bool with_headers = true, bool headers_only = false) {
     if (obs_all_cells_in_regs<NIT, TURN>() && view_count > NIT * 32)
         mg::fatal("render kernel NIT=%d chosen for a view of %d in-range cells", NIT, view_count);
     if ((size_t)n_total > c->obs_hdr_n) {                                // scratch owned by the context: per-agent headers
@@ -1310,15 +1322,17 @@ static void launch_obs_typed(Ctx *c, int cfg_slot, const EngineDev &hE, ObsParam
     }
     if (headers_only) return;
     // the wide tile whenever it keeps at least as many warps per SM as the narrow one (always, for battle); the
-    // narrow tile for records whose wide tile fits fewer warps or not at all
+    // narrow tile for records whose wide tile fits fewer warps or not at all.  O.tile forces a width: 1 narrow, 2 wide
+    // (narrow when the wide tile does not fit).
     constexpr int TN = obs_tile_narrow<T>(), TW = obs_tile_wide<T>();
     const size_t lut_bytes = (size_t)(P.turn ? 4 : 1) * ((P.cells + 1) & ~1) * sizeof(int2);
     const size_t smem_n = (size_t)TN * P.rec * sizeof(T) + lut_bytes, smem_w = (size_t)TW * P.rec * sizeof(T) + lut_bytes;
     if (smem_n > 227 * 1024) mg::fatal("observation record too large for the render kernel (%zu bytes of shared memory)", smem_n);
     const int ctas_w = obs_ctas_per_sm<T, NIT, TURN, TW>(c, 2 * cfg_slot + 1, smem_w);
     const int ctas_n = obs_ctas_per_sm<T, NIT, TURN, TN>(c, 2 * cfg_slot, smem_n);
-    if (ctas_w >= 1 && ctas_w * TW >= ctas_n * TN) launch_obs_render<T, NIT, TURN, TW>(c, P, n_total, smem_w, ctas_w);
-    else launch_obs_render<T, NIT, TURN, TN>(c, P, n_total, smem_n, ctas_n < 1 ? 1 : ctas_n);
+    const bool wide = O.tile == 0 ? ctas_w >= 1 && ctas_w * TW >= ctas_n * TN : O.tile == 2 && ctas_w >= 1;
+    if (wide) launch_obs_render<T, NIT, TURN, TW>(c, O, P, n_total, smem_w, ctas_w);
+    else launch_obs_render<T, NIT, TURN, TN>(c, O, P, n_total, smem_n, ctas_n < 1 ? 1 : ctas_n);
 }
 
 static void fill_obs_params(Ctx *c, const EngineDev &hE, const ObsArgs &O, const float *mm_val, int n_total, ObsParams &P) {
@@ -1352,14 +1366,14 @@ static void launch_obs_dispatch(Ctx *c, const EngineDev &hE, const ObsArgs &O, O
     const int vc = hE.grp[O.group].view_count;
     const bool small_view = vc <= 4 * 32;                       // in-range view cells held in registers: 4 or 8 per lane
     if (hE.turn_mode) {                                         // headings: per-heading LUTs in shared memory (NIT = 8 code path)
-        if (O.half) launch_obs_typed<__half, 8, true>(c, 0, hE, P, n_total, vc, with_headers, headers_only);
-        else launch_obs_typed<float, 8, true>(c, 1, hE, P, n_total, vc, with_headers, headers_only);
+        if (O.half) launch_obs_typed<__half, 8, true>(c, 0, hE, O, P, n_total, vc, with_headers, headers_only);
+        else launch_obs_typed<float, 8, true>(c, 1, hE, O, P, n_total, vc, with_headers, headers_only);
     } else if (O.half) {
-        if (small_view) launch_obs_typed<__half, 4, false>(c, 2, hE, P, n_total, vc, with_headers, headers_only);
-        else launch_obs_typed<__half, 8, false>(c, 3, hE, P, n_total, vc, with_headers, headers_only);
+        if (small_view) launch_obs_typed<__half, 4, false>(c, 2, hE, O, P, n_total, vc, with_headers, headers_only);
+        else launch_obs_typed<__half, 8, false>(c, 3, hE, O, P, n_total, vc, with_headers, headers_only);
     } else {
-        if (small_view) launch_obs_typed<float, 4, false>(c, 4, hE, P, n_total, vc, with_headers, headers_only);
-        else launch_obs_typed<float, 8, false>(c, 5, hE, P, n_total, vc, with_headers, headers_only);
+        if (small_view) launch_obs_typed<float, 4, false>(c, 4, hE, O, P, n_total, vc, with_headers, headers_only);
+        else launch_obs_typed<float, 8, false>(c, 5, hE, O, P, n_total, vc, with_headers, headers_only);
     }
 }
 
@@ -1369,6 +1383,8 @@ void launch_obs(Ctx *c, const EngineDev *, const EngineDev &hE, const ObsArgs &O
     fill_obs_params(c, hE, O, mm_val, n_total, P);
     launch_obs_dispatch(c, hE, O, P, n_total, true, false);
 }
+
+void obs_launch_report(const Ctx *c, int out[8]) { memcpy(out, c->obs_last, sizeof c->obs_last); }
 
 // ------------------------------------------------------------------------------------------------
 // global state (magent_b200_get_global_state): state_compose_cell of every map cell of every arena, [A][H][W][C] in T.

@@ -228,6 +228,9 @@ struct ObsArgs {
     void *view;                               // [sum_a n][view_h][view_w][n_channel]
     void *feature;                            // [sum_a n][feature_size]
     int half;                                 // 0: float32 (reference ABI), 1: IEEE half (compact hand-off)
+    // render launch shape forced by the engine's "obs_grid" / "obs_chunk" / "obs_tile" keys (0: automatic); the backend
+    // clamps grid to [1, tiles] and chunk to [1, ceil(tiles / grid)]; tile 1 = narrow, 2 = wide (narrow when it does not fit)
+    int grid = 0, chunk = 0, tile = 0;
 };
 
 enum InfoKind { INFO_ID = 0, INFO_POS, INFO_ALIVE, INFO_REWARD, INFO_ACTION_SCATTER, INFO_HP };

@@ -148,7 +148,7 @@ int Engine::feature_size(int g) const {              // GridWorld.cc:926-934
     return f;
 }
 
-void Engine::set_config(const char *key, void *p_value) {     // GridWorld.cc:120-149
+int Engine::set_config(const char *key, void *p_value) {      // GridWorld.cc:120-149
     int ivalue = *(int *)p_value;
     bool bvalue = *(bool *)p_value;
     if (strequ(key, "map_width")) W_ = ivalue;
@@ -178,7 +178,15 @@ void Engine::set_config(const char *key, void *p_value) {     // GridWorld.cc:12
     } else if (strequ(key, "device_id")) device_id_ = ivalue;
     else if (strequ(key, "host_path")) host_path_ = ivalue;               // 1 wire records + host expansion (default for large
                                                                            // observations), 0 dense DMA, 2 wire whatever the size
+    // render launch shape of this engine's observations (0: automatic): CTAs, consecutive tiles per CTA visit, tile
+    // width 1 narrow / 2 wide.  Tests use them to make every CTA render many tiles at small sizes.
+    else if (strequ(key, "obs_grid") || strequ(key, "obs_chunk") || strequ(key, "obs_tile")) {
+        const bool tile = strequ(key, "obs_tile");
+        if (ivalue < 0 || (tile && ivalue > 2)) return refuse("%s = %d: must be %s", key, ivalue, tile ? "0, 1 or 2" : ">= 0");
+        (strequ(key, "obs_grid") ? obs_grid_ : tile ? obs_tile_ : obs_chunk_) = ivalue;
+    }
     else fatal("invalid argument in GridWorld::set_config : %s", key);
+    return 0;
 }
 
 void Engine::register_agent_type(const char *name, int n, const char **keys, float *values) {
@@ -951,6 +959,7 @@ void Engine::get_observation(int group, void **bufs, int half) {      // GridWor
     }
     ObsArgs O;
     O.curmask = curmask_; O.group = group; O.half = half ? 1 : 0;
+    O.grid = obs_grid_; O.chunk = obs_chunk_; O.tile = obs_tile_;
     if (vdev) O.view = bufs[0];
     else { stage_reserve(d_view_stage_, view_stage_bytes_, vbytes); O.view = d_view_stage_; }
     if (fdev) O.feature = bufs[1];
@@ -1451,11 +1460,21 @@ int Engine::get_counters(long long *out, int cap) {
     return n;
 }
 
-void Engine::get_info(int group, const char *name, void *void_buffer) {        // GridWorld.cc:709-894
+int Engine::get_info(int group, const char *name, void *void_buffer) {         // GridWorld.cc:709-894
     int *ib = (int *)void_buffer;
+    if (strequ(name, "obs_override")) {                 // extension: the obs_grid, obs_chunk, obs_tile keys
+        ib[0] = obs_grid_; ib[1] = obs_chunk_; ib[2] = obs_tile_;
+        return 0;
+    }
+    if (strequ(name, "obs_launch")) {                   // extension: shape of this engine's last render launch
+        if (!be::obs_launch_report) return refuse("the %s backend does not report its render launches", be::name());
+        for (int i = 0; i < 8; ++i) ib[i] = 0;
+        if (bx_) be::obs_launch_report(bx_, ib);
+        return 0;
+    }
     if (strequ(name, "state_space")) {                  // extension: per-arena shape of magent_b200_get_global_state
         ib[0] = H_; ib[1] = W_; ib[2] = state_channels();               // fixed: no counts needed, nothing to wait for
-        return;
+        return 0;
     }
     if (strequ(name, "num_bound")) {                    // extension: per group, records a device-pointer call may write
         const std::vector<int> floor = restore_floor(); // before the counts next settle (no waiting here)
@@ -1464,7 +1483,7 @@ void Engine::get_info(int group, const char *name, void *void_buffer) {        /
             for (int a = 0; a < A_; ++a) n += std::max(count(g, a), floor[g]);
             ib[g] = (int)n;
         }
-        return;
+        return 0;
     }
     if (strequ(name, "arena_rng")) {                    // extension: uint32 minstd state of every arena
         if (where_ == DEVICE) {
@@ -1474,7 +1493,7 @@ void Engine::get_info(int group, const char *name, void *void_buffer) {        /
         } else {
             for (int a = 0; a < A_; ++a) ((uint32_t *)void_buffer)[a] = arenas_[a].rng;
         }
-        return;
+        return 0;
     }
     settle_counts();
     float *fb = (float *)void_buffer;
@@ -1485,10 +1504,10 @@ void Engine::get_info(int group, const char *name, void *void_buffer) {        /
         check_group(group, "get_info");
         to_device();
         const int n = total(group);
-        if (n == 0) return;
+        if (n == 0) return 0;
         int kind = strequ(name, "id") ? INFO_ID : strequ(name, "pos") ? INFO_POS : strequ(name, "alive") ? INFO_ALIVE : INFO_HP;
         size_t bytes = kind == INFO_POS ? (size_t)n * 8 : kind == INFO_ALIVE ? (size_t)n : (size_t)n * 4;
-        if (be::is_device_ptr(void_buffer)) { be::launch_info(bx_, dE_, hE_, curmask_, kind, group, void_buffer, n); return; }
+        if (be::is_device_ptr(void_buffer)) { be::launch_info(bx_, dE_, hE_, curmask_, kind, group, void_buffer, n); return 0; }
         void *st = io_stage(bytes);
         be::launch_info(bx_, dE_, hE_, curmask_, kind, group, st, n);
         be::d2h(bx_, void_buffer, st, bytes);
@@ -1583,6 +1602,7 @@ void Engine::get_info(int group, const char *name, void *void_buffer) {        /
     } else {
         fatal("unsupported info name in GridWorld::get_info : %s", name);
     }
+    return 0;
 }
 
 }  // namespace mg

@@ -88,7 +88,7 @@ public:
     ~Engine();
 
     // ---- reference Environment / GridWorld surface
-    void set_config(const char *key, void *p_value);
+    int set_config(const char *key, void *p_value);     // -1: refused (extension keys; last_error says why)
     void register_agent_type(const char *name, int n, const char **keys, float *values);
     void new_group(const char *type_name, int *handle);
     void define_agent_symbol(int no, int group, int index);
@@ -102,7 +102,7 @@ public:
     void step(int *done);
     void get_reward(int group, float *buf);
     void clear_dead();
-    void get_info(int group, const char *name, void *buf);
+    int get_info(int group, const char *name, void *buf);   // -1: refused (extension keys)
     void set_goal(int group, const char *method, const int *buf);
     void render();
 
@@ -181,6 +181,7 @@ private:
     long long io_[IO_N] = {0, 0, 0, 0, 0, 0};       // step-loop traffic (hot calls only) and host-path phase times
     bool done_stale_ = false;           // arenas_[a].done not refreshed by the last step (device-pointer done)
     int host_path_ = -1;                // env_get_observation into host memory: 1 wire records + host expansion, 0 dense DMA
+    int obs_grid_ = 0, obs_chunk_ = 0, obs_tile_ = 0;   // forced render launch shape (ObsArgs; 0: automatic)
     unsigned long long rand_calls_ = 0;
     // get_observation pre-pass products (hp_norm plane, minimap) stay valid until the state changes
     unsigned long long state_version_ = 1, prep_version_ = 0;

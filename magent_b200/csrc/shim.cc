@@ -32,13 +32,13 @@ MG_API int env_new_game(EnvHandle *game, const char *name) {
     return 0;
 }
 MG_API int env_delete_game(EnvHandle game) { delete E(game); return 0; }
-MG_API int env_config_game(EnvHandle game, const char *name, void *p_value) { E(game)->set_config(name, p_value); return 0; }
+MG_API int env_config_game(EnvHandle game, const char *name, void *p_value) { return E(game)->set_config(name, p_value); }
 MG_API int env_reset(EnvHandle game) { E(game)->reset(); return 0; }
 MG_API int env_get_observation(EnvHandle game, GroupHandle group, float **buffer) { E(game)->get_observation(group, (void **)buffer, 0); return 0; }
 MG_API int env_set_action(EnvHandle game, GroupHandle group, const int *actions) { E(game)->set_action(group, actions); return 0; }
 MG_API int env_step(EnvHandle game, int *done) { E(game)->step(done); return 0; }
 MG_API int env_get_reward(EnvHandle game, GroupHandle group, float *buffer) { E(game)->get_reward(group, buffer); return 0; }
-MG_API int env_get_info(EnvHandle game, GroupHandle group, const char *name, void *buffer) { E(game)->get_info(group, name, buffer); return 0; }
+MG_API int env_get_info(EnvHandle game, GroupHandle group, const char *name, void *buffer) { return E(game)->get_info(group, name, buffer); }
 MG_API int env_render(EnvHandle game) { E(game)->render(); return 0; }
 MG_API int env_render_next_file(EnvHandle game) { E(game)->render_next_file(); return 0; }
 

@@ -94,6 +94,7 @@ class GridWorld(Environment):
         self.num_arenas = int(kwargs.pop("_num_arenas", 1))
         device = kwargs.pop("_device", None)
         host_path = kwargs.pop("_host_path", None)      # None: engine default (wire); "dense": dense records over PCIe
+        obs_launch = kwargs.pop("_obs_launch", None)    # (grid, chunk, tile) of the observation render; 0 = automatic
         self.game = None
 
         if isinstance(config, str):
@@ -128,6 +129,10 @@ class GridWorld(Environment):
             # "dense": dense records over PCIe; "wire": wire records + host expansion whatever the size; default: wire for
             # observations of 16 MB and more, dense below
             L.env_config_game(game, b"host_path", _cint({"dense": 0, "wire": 2, "auto": 1}[host_path]))
+        if obs_launch is not None:
+            if not L.is_b200:
+                raise ValueError("_obs_launch needs the B200 engine library")
+            self._set_obs_launch(*obs_launch)
 
         for key, value in config.config_dict.items():
             kind = self._CONFIG_TYPES[key]
@@ -600,6 +605,31 @@ class GridWorld(Environment):
         n = ctypes.c_longlong(0)
         self._lib.magent_b200_get_profile(self.game, ctypes.byref(ms), ctypes.byref(n))
         return ms.value, n.value
+
+    def _set_obs_launch(self, grid=0, chunk=0, tile=0):
+        """force the observation render's launch shape of this engine (tests): CTAs, consecutive tiles per CTA visit,
+        tile width 1 narrow / 2 wide; 0 = automatic.  Raises ValueError (and changes nothing) on a refused value."""
+        keys = (b"obs_grid", b"obs_chunk", b"obs_tile")
+        old = self._get_obs_override()
+        for key, value in zip(keys, (grid, chunk, tile)):
+            if self._lib.env_config_game(self.game, key, _cint(int(value))) < 0:
+                why = self._lib.magent_b200_last_error().decode()
+                for k, v in zip(keys, old):
+                    self._lib.env_config_game(self.game, k, _cint(v))
+                raise ValueError(why)
+
+    def _get_obs_override(self):
+        """(grid, chunk, tile) as set by _set_obs_launch"""
+        buf = np.zeros((3,), dtype=np.int32)
+        self._lib.env_get_info(self.game, -1, b"obs_override", buf.ctypes.data)
+        return tuple(int(v) for v in buf)
+
+    def _get_obs_launch(self):
+        """the last render launch of this engine: dict(elem_bytes, nit, turn, tile_agents, grid, chunk, tiles, aligned)"""
+        buf = np.zeros((8,), dtype=np.int32)
+        self._check(self._lib.env_get_info(self.game, -1, b"obs_launch", buf.ctypes.data), "obs_launch")
+        keys = ("elem_bytes", "nit", "turn", "tile_agents", "grid", "chunk", "tiles", "aligned")
+        return dict(zip(keys, (int(v) for v in buf)))
 
     def launch_count(self):
         """number of kernels this library has launched in this process"""
