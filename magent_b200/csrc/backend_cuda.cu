@@ -1158,7 +1158,9 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
             const long o2 = (long)tile2 * OBS_TA + warp;
             if (o2 < n_total) hA2 = P.hdr[o2];
         }
-        // the previous tile's bulk store must have finished READING the buffer before it is touched
+        // the previous tile's bulk store must have finished READING the buffer before it is touched.  One buffer per
+        // CTA on purpose: a second would cost a CTA per SM, and at battle's size that loses more than the overlap
+        // wins (DESIGN.md section 5, "Two tile slots per CTA")
         if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
         __syncthreads();
         if (active && !(OBS_ABLATE & 2)) {
@@ -1242,8 +1244,13 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
         const unsigned bytes = (unsigned)cnt * (unsigned)P.rec * (unsigned)sizeof(T);
         if ((bytes & 15u) == 0 && (((size_t)gout) & 15) == 0) {
             if (threadIdx.x == 0 && !(OBS_ABLATE & 8)) {
-                asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                             :: "l"(gout), "r"(smem_u32(buf)), "r"(bytes) : "memory");
+                // the output is a write-once stream far larger than L2: evict_first keeps it from pushing out the
+                // planes, minimap rows and headers the composition reads (the policy is made here, not held in a
+                // register across the loop)
+                unsigned long long pol;
+                asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+                asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
+                             :: "l"(gout), "r"(smem_u32(buf)), "r"(bytes), "l"(pol) : "memory");
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }
         } else {                                   // ragged last tile / unaligned caller buffer
