@@ -30,6 +30,25 @@ int magent_b200_select_arena(EnvHandle game, int arena);
 /* set_action with uniform random actions generated on the device (throughput runs; not part of parity).
  * `unused` must be NULL. */
 int magent_b200_random_actions(EnvHandle game, GroupHandle group, void *unused, unsigned long long seed);
+/* legal-action mask: uint8 [n][n_action] in ABI order (the rows of env_set_action, un-culled dead agents included).
+ * Byte [i][k] is 1 iff action k, taken by agent i alone on the state as it is now, would succeed:
+ *   move    the target footprint is inside the board by the reference's own test, free of walls and food, and every cell
+ *           is empty or the mover's own (the centre move of a live agent is therefore always 1); or the first other
+ *           agent in the blocked footprint is an absorbing type that has not absorbed yet (the mover would be swallowed)
+ *   turn    (turn_mode) the rotated footprint is free or the agent's own
+ *   attack  the aimed cell is on the board and holds an agent of another group, of the own group when the type has
+ *           attack_in_group, or food (food_mode)
+ * What other agents do in the same step is not anticipated.  A dead, un-culled agent has an all-zero row; an absorbed
+ * absorber has no legal move (its turns and attacks are decided as for anyone else).  Returns -1 for a bad group handle.
+ * Host pointer or CUDA device pointer.  With a device pointer: no synchronisation, no allocation, recordable into a CUDA
+ * graph; rows are sized by the device-side counts, at most "num_bound" of them are written.  magent_b200_select_arena
+ * does not apply. */
+int magent_b200_get_action_mask(EnvHandle game, GroupHandle group, unsigned char *buffer);
+/* set_action with an action drawn uniformly from the legal actions (the mask above) of every agent, on the device; an
+ * agent without a legal action gets action 0, which the step ignores for it.  Same seeding discipline as
+ * magent_b200_random_actions: the call counter of both calls and the device step counter ride in the seed, so a replayed
+ * graph draws fresh actions.  Not part of parity.  Returns -1 for a bad group handle. */
+int magent_b200_random_legal_actions(EnvHandle game, GroupHandle group, unsigned long long seed);
 /* compact observation hand-off (SURVEY.md 8f rank 2): same call, layout and pointer rules as env_get_observation
  * (reference src/runtime_api.h:35), but every element is an IEEE binary16 = the float32 value rounded to
  * nearest-even.  buffer[0] = view [n][view_h][view_w][n_channel], buffer[1] = feature [n][feature_size];

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libmagent.so")
 SOURCES = ["engine.cc", "shim.cc", "host_expand.cc", "backend_cuda.cu"]
-HEADERS = ["hd.h", "dev_types.h", "step_phases.h", "obs_phases.h", "backend.h", "engine.h", "host_expand.h",
+HEADERS = ["hd.h", "dev_types.h", "step_phases.h", "obs_phases.h", "mask_phases.h", "backend.h", "engine.h", "host_expand.h",
            os.path.join("..", "..", "include", "magent_runtime_api.h"),
            os.path.join("..", "..", "include", "magent_b200_ext.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -63,6 +63,8 @@ EXT_SIGNATURES = {
     "magent_b200_sync": ([_vp], ctypes.c_int),
     "magent_b200_select_arena": ([_vp, ctypes.c_int], ctypes.c_int),
     "magent_b200_random_actions": ([_vp, ctypes.c_int, _vp, ctypes.c_ulonglong], ctypes.c_int),
+    "magent_b200_get_action_mask": ([_vp, ctypes.c_int, _vp], ctypes.c_int),
+    "magent_b200_random_legal_actions": ([_vp, ctypes.c_int, ctypes.c_ulonglong], ctypes.c_int),
     "magent_b200_get_observation_f16": ([_vp, ctypes.c_int, ctypes.POINTER(_vp)], ctypes.c_int),
     "magent_b200_get_global_state": ([_vp, _vp, ctypes.c_int], ctypes.c_int),
     "magent_b200_snapshot_arenas": ([_vp], ctypes.c_int),

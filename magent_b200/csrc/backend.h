@@ -72,6 +72,14 @@ void launch_info(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curma
                  void *buf, int n_total);
 void launch_random_actions(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group,
                            unsigned long long seed, int n_total);
+// Legal actions of every agent of `group` (mask_phases.h action_legal).  launch_action_mask: uint8 [n][n_action] into
+// `out`, a device buffer; launch_random_legal_actions: AgentSoA::act of every agent drawn uniformly from its legal actions
+// (mask_phases.h legal_draw; 0 when it has none).  n_total is the host's count, an upper bound: the device-side offsets
+// decide.  Declared weak like launch_global_state: a backend without them loads, and the engine refuses the calls.
+__attribute__((weak)) void launch_action_mask(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group,
+                                              unsigned char *out, int n_total);
+__attribute__((weak)) void launch_random_legal_actions(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask,
+                                                       int group, unsigned long long seed, int n_total);
 // clear_dead: asynchronous read-back of the [G][A+1] offset table (launch_offsets) into page-locked memory
 void counts_fetch_begin(Ctx *, const int *dev_off, size_t n_ints);
 const int *counts_fetch_wait(Ctx *);     // blocks until the fetch has landed; valid until the next counts_fetch_begin

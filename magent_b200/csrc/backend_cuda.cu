@@ -27,6 +27,7 @@
 namespace mg { __device__ long long mg_phase_clock[8 * 32]; }
 #endif
 #include "obs_phases.h"
+#include "mask_phases.h"
 
 namespace cg = cooperative_groups;
 
@@ -695,13 +696,6 @@ void launch_info(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curm
     post_launch("info_kernel");
 }
 
-__device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
-    x += 0x9E3779B97F4A7C15ull;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-    return x ^ (x >> 31);
-}
-
 __global__ void __launch_bounds__(256) random_actions_kernel(const EngineDev *gE, unsigned curmask, int g,
                                                              unsigned long long seed, int n_total, int chunks_per_arena) {
     const EngineDev &E = *gE;
@@ -726,6 +720,126 @@ void launch_random_actions(Ctx *c, const EngineDev *dE, const EngineDev &hE, uns
     const int cpa = (cap + threads - 1) / threads;
     random_actions_kernel<<<(unsigned)((size_t)hE.A * cpa), threads, 0, c->stream>>>(dE, curmask, group, seed, n_total, cpa);
     post_launch("random_actions_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
+// legal-action mask (magent_b200_get_action_mask) and legal draws (magent_b200_random_legal_actions): mask_phases.h
+// action_legal for every (agent, action) of a group.  CTAs are dealt per arena like info_kernel (blockIdx says which
+// arena, the device-side offsets decide how many agents it has, the host's count is only an upper bound).  A CTA owns
+// MASK_THREADS consecutive agents.  In the mask kernel a warp takes 32 of them: lane j loads agent j's own fields
+// (coalesced), then the warp visits its agents one after the other with the lanes spread over the actions, every lane
+// deciding one action per 32 from one to a handful of cells of the arena's `occ` plane (an L2 hit: a plane is
+// 40-200 KB).
+constexpr int MASK_THREADS = 256;
+
+struct MaskWarp {                    // the agents of one warp: lane j holds agent i0 + j
+    int a, g, o0, c0, i0, cnt;       // arena, group, the arena's first ABI row, first agent of the CTA / of the warp
+    MaskAgent mine;
+    __device__ __forceinline__ MaskAgent agent(int j) const {
+        MaskAgent m;
+        m.x = __shfl_sync(0xffffffffu, mine.x, j); m.y = __shfl_sync(0xffffffffu, mine.y, j);
+        m.dir = __shfl_sync(0xffffffffu, mine.dir, j); m.code = code_make(g, i0 + j);
+        m.flags = (unsigned char)__shfl_sync(0xffffffffu, (int)mine.flags, j);
+        return m;
+    }
+};
+// returns the number of agents of the CTA (the same in every thread of it)
+__device__ __forceinline__ int mask_warp_setup(const EngineDev &E, unsigned curmask, int g, int n_total, int chunks_per_arena,
+                                               MaskWarp &w) {
+    const int *off = E.off + (size_t)g * (E.A + 1);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    w.g = g;
+    w.a = blockIdx.x / chunks_per_arena;
+    const int c0 = w.c0 = (blockIdx.x - w.a * chunks_per_arena) * MASK_THREADS;
+    w.o0 = off[w.a];
+    int cta_cnt = min(MASK_THREADS, off[w.a + 1] - w.o0 - c0);
+    cta_cnt = min(cta_cnt, n_total - (w.o0 + c0));               // never beyond the caller's buffer
+    w.i0 = c0 + 32 * warp;
+    w.cnt = min(32, cta_cnt - 32 * warp);
+    w.mine.x = w.mine.y = 0; w.mine.dir = DIR_NORTH; w.mine.code = 0; w.mine.flags = FLAG_DEAD;
+    if (lane < w.cnt) w.mine = mask_agent(E, curmask, w.a, g, w.i0 + lane);
+    return cta_cnt;
+}
+
+__global__ void __launch_bounds__(MASK_THREADS) action_mask_kernel(const EngineDev *gE, unsigned curmask, int g,
+                                                                  unsigned char *out, int n_total, int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    extern __shared__ __align__(16) unsigned char mask_smem[];
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    MaskWarp w;
+    const int cta_cnt = mask_warp_setup(E, curmask, g, n_total, chunks_per_arena, w);
+    if (cta_cnt <= 0) return;
+    const int na = E.grp[g].n_action, lane = threadIdx.x & 31;
+    // the CTA's rows are one contiguous byte range of the output: composed in shared memory at the same offset from a
+    // 16-byte boundary as their destination, so that the body of the copy below is 16 bytes per thread on both sides
+    unsigned char *dst = out + (size_t)(w.o0 + w.c0) * na;
+    const int shift = (int)((size_t)dst & 15);
+    unsigned char *rows = mask_smem + shift;
+    const int *occ = E.occ + (long)w.a * E.W * E.H;
+    for (int j = 0; j < w.cnt; ++j) {
+        const MaskAgent m = w.agent(j);
+        unsigned char *row = rows + (size_t)(w.i0 - w.c0 + j) * na;
+        for (int k = lane; k < na; k += 32) row[k] = action_legal(E, curmask, w.a, occ, g, m, k) ? 1 : 0;
+    }
+    __syncthreads();
+    const int total = cta_cnt * na;
+    const int head = min(total, (16 - shift) & 15);
+    const int body = (total - head) >> 4;
+    for (int q = threadIdx.x; q < head; q += MASK_THREADS) dst[q] = rows[q];
+    for (int q = threadIdx.x; q < body; q += MASK_THREADS) ((uint4 *)(dst + head))[q] = ((const uint4 *)(rows + head))[q];
+    for (int q = head + (body << 4) + threadIdx.x; q < total; q += MASK_THREADS) dst[q] = rows[q];
+}
+
+// The byte mask is never materialised: one thread per agent counts its legal actions, draws r = legal_draw(...) below
+// that count and walks to the r-th legal action in ascending action order.  The walk decides the same cells again; they
+// are L1 hits by then.  No legal action (dead, or an absorbed absorber with nothing to attack): action 0, which the step
+// ignores for such an agent.
+__global__ void __launch_bounds__(MASK_THREADS) random_legal_actions_kernel(const EngineDev *gE, unsigned curmask, int g,
+                                                                           unsigned long long seed, int n_total,
+                                                                           int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int *off = E.off + (size_t)g * (E.A + 1);
+    const int a = blockIdx.x / chunks_per_arena;
+    const int i = (blockIdx.x - a * chunks_per_arena) * MASK_THREADS + threadIdx.x;
+    const int o0 = off[a];
+    const int o = o0 + i;
+    if (i >= off[a + 1] - o0 || o >= n_total) return;
+    const int na = E.grp[g].n_action;
+    const int *occ = E.occ + (long)a * E.W * E.H;
+    const MaskAgent m = mask_agent(E, curmask, a, g, i);
+    int n_legal = 0;
+    for (int k = 0; k < na; ++k) n_legal += action_legal(E, curmask, a, occ, g, m, k) ? 1 : 0;
+    int act = 0;
+    if (n_legal > 0) {
+        int r = legal_draw(seed, E.counters[CNT_STEPS], o, n_legal);
+        for (; r >= 0; ++act) r -= action_legal(E, curmask, a, occ, g, m, act) ? 1 : 0;
+        --act;
+    }
+    cur_soa(E, curmask, g).act[gidx(E, a, g, i)] = act;
+}
+
+static int mask_chunks_per_arena(const EngineDev &hE, int group) { return (hE.grp[group].cap + MASK_THREADS - 1) / MASK_THREADS; }
+
+void launch_action_mask(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group, unsigned char *out,
+                        int n_total) {
+    DeviceGuard guard(c);
+    const int na = hE.grp[group].n_action;
+    const size_t smem = (size_t)MASK_THREADS * na + 16;
+    if (smem + sizeof(EngineDev) > 48 * 1024) mg::fatal("action mask: %d actions per agent are more than the kernels hold", na);
+    const int cpa = mask_chunks_per_arena(hE, group);
+    action_mask_kernel<<<(unsigned)((size_t)hE.A * cpa), MASK_THREADS, smem, c->stream>>>(dE, curmask, group, out, n_total, cpa);
+    post_launch("action_mask_kernel");
+}
+
+void launch_random_legal_actions(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group,
+                                 unsigned long long seed, int n_total) {
+    DeviceGuard guard(c);
+    const int cpa = mask_chunks_per_arena(hE, group);
+    random_legal_actions_kernel<<<(unsigned)((size_t)hE.A * cpa), MASK_THREADS, 0, c->stream>>>(dE, curmask, group, seed, n_total, cpa);
+    post_launch("random_legal_actions_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1211,6 +1211,38 @@ void Engine::random_actions(int group, unsigned long long seed) {
     be::launch_random_actions(bx_, dE_, hE_, curmask_, group, seed * 0x9E3779B97F4A7C15ull + (++rand_calls_), n);
 }
 
+// Legal-action mask of one group.  A device buffer takes one kernel sized by the host's (upper-bound) counts and clamped
+// by the device's: no synchronisation, no allocation, recordable into a graph.  A host buffer needs the exact counts and
+// goes through the i/o staging like the other per-agent read-backs.
+int Engine::get_action_mask(int group, unsigned char *buf) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_action_mask", group);
+    if (!be::launch_action_mask) return refuse("the %s backend has no action-mask kernel", be::name());
+    to_device();
+    const bool dev = be::is_device_ptr(buf);
+    if (!dev) settle_counts();
+    const int n = total(group);
+    if (n == 0) return 0;
+    if (dev) { be::launch_action_mask(bx_, dE_, hE_, curmask_, group, buf, n); return 0; }
+    const size_t bytes = (size_t)n * group_type_[group]->n_action;
+    unsigned char *st = (unsigned char *)io_stage(bytes);
+    be::launch_action_mask(bx_, dE_, hE_, curmask_, group, st, n);
+    be::d2h(bx_, buf, st, bytes);
+    io_[IO_D2H] += (long long)bytes;
+    return 0;
+}
+
+int Engine::random_legal_actions(int group, unsigned long long seed) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in random_legal_actions", group);
+    if (!be::launch_random_legal_actions) return refuse("the %s backend has no legal-action sampler", be::name());
+    to_device();
+    if (std::find(order_.begin(), order_.end(), group) == order_.end()) order_.push_back(group);
+    const int n = total(group);
+    if (n == 0) return 0;
+    // the seed the kernel sees (mask_phases.h legal_draw): shares the call counter of random_actions
+    be::launch_random_legal_actions(bx_, dE_, hE_, curmask_, group, seed * 0x9E3779B97F4A7C15ull + (++rand_calls_), n);
+    return 0;
+}
+
 void Engine::step(int *done) {                                        // GridWorld.cc:456-631
     to_device();
     StepArgs S;

@@ -119,6 +119,10 @@ public:
     int free_snapshot(int id);
     int restore_arenas(int id, const int *src, int keep_rng);
     int get_arena_done(int *out);
+    // legal actions (mask_phases.h): uint8 [n][n_action] of one group / actions drawn uniformly from them on the device.
+    // -1 and the last error when refused.
+    int get_action_mask(int group, unsigned char *buf);
+    int random_legal_actions(int group, unsigned long long seed);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads

@@ -101,6 +101,12 @@ MG_API int magent_b200_select_arena(EnvHandle game, int arena) { E(game)->select
 MG_API int magent_b200_random_actions(EnvHandle game, GroupHandle group, void *, unsigned long long seed) {
     E(game)->random_actions(group, seed); return 0;
 }
+MG_API int magent_b200_get_action_mask(EnvHandle game, GroupHandle group, unsigned char *buffer) {
+    return E(game)->get_action_mask(group, buffer);
+}
+MG_API int magent_b200_random_legal_actions(EnvHandle game, GroupHandle group, unsigned long long seed) {
+    return E(game)->random_legal_actions(group, seed);
+}
 MG_API int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **buffer) {
     E(game)->get_observation(group, buffer, 1);
     return 0;

@@ -516,6 +516,29 @@ MG_HD void mover_dims(const EngineDev &E, const GroupDev &G, const AgentSoA &s, 
 // -1 nor 1: Map::do_turn takes its "else" formula and new_dir = (dir + wise + 4) % 4, Map.cc:367)
 MG_HD int turned_dir(int dir, int act) { return (dir + 2 * act - 1 + 4) % 4; }
 
+// Where a move (turn == false) or turn (turn == true) action `act` would put an agent at (x, y) facing `dir`: top-left
+// corner (nx, ny) and footprint bw x bh.  Returns the reference's in-board verdict for that footprint (Map.cc:455).
+// Shared by the step (phase_move_register) and the legal-action mask (mask_phases.h).
+MG_HD bool mover_target(const EngineDev &E, const GroupDev &G, int act, int x, int y, int dir, bool turn,
+                        int &nx, int &ny, int &bw, int &bh) {
+    if (turn) {
+        // the body pivots about its "real" corner (turn offsets are 0, AgentType.cc:108): the stored top-left
+        // corner follows from real_to_save with the new direction
+        const int nd = turned_dir(dir, act);
+        int rx, ry, qx, qy;
+        dir_real(G, dir, rx, ry);
+        dir_real(G, nd, qx, qy);
+        nx = x + rx - qx; ny = y + ry - qy;
+    } else {
+        int dx = ld_ro(G.move_dx + act), dy = ld_ro(G.move_dy + act);
+        if (E.turn_mode) { const int rx = dx, ry = dy; dir_rot(dir, rx, ry, dx, dy); }     // GridWorld.cc:587-598
+        nx = x + dx; ny = y + dy;
+    }
+    body_dims(G, dir, bw, bh);
+    if (turn) { int t = bw; bw = bh; bh = t; }       // every turn is by 90 degrees
+    return !(nx < 0 || ny < 0 || nx + bw >= E.W || ny + bh >= E.H);
+}
+
 // phase 6: movers (turn == false) or turners (turn == true, turn_mode only) compute their target footprint and
 // queue on every target cell.  Turn: Map::do_turn, Map.cc:361-406; move: Map::do_move, Map.cc:313-358.
 // A thread owns ~4 movers.  One at a time each costs three dependent global round trips (own fields -> occupancy of
@@ -566,25 +589,10 @@ MG_HD void phase_move_register(Ctx &c, const EngineDev &E, const StepArgs &S, in
                 if (!(xm < 4 || xm > E.bandwidth - 4)) bucket = (unsigned)(x[u] / E.bandwidth);
             }
             E.mv_key[f] = (bucket << 27) | ((unsigned)k << 23) | (unsigned)i;
-            int nx, ny;
-            if (turn) {
-                // the body pivots about its "real" corner (turn offsets are 0, AgentType.cc:108): the stored top-left
-                // corner follows from real_to_save with the new direction
-                const int nd = turned_dir(dir[u], av);
-                int rx, ry, qx, qy;
-                dir_real(G, dir[u], rx, ry);
-                dir_real(G, nd, qx, qy);
-                nx = x[u] + rx - qx; ny = y[u] + ry - qy;
-            } else {
-                int dx = ld_ro(G.move_dx + av), dy = ld_ro(G.move_dy + av);
-                if (E.turn_mode) { const int rx = dx, ry = dy; dir_rot(dir[u], rx, ry, dx, dy); }     // GridWorld.cc:587-598
-                nx = x[u] + dx; ny = y[u] + dy;
-            }
+            int nx, ny, bw, bh;
+            const bool in_board = mover_target(E, G, av, x[u], y[u], dir[u], turn, nx, ny, bw, bh);
             E.mv_nx[f] = nx; E.mv_ny[f] = ny;
-            int bw, bh;
-            body_dims(G, dir[u], bw, bh);
-            if (turn) { int t = bw; bw = bh; bh = t; }   // every turn is by 90 degrees
-            if (nx < 0 || ny < 0 || nx + bw >= E.W || ny + bh >= E.H) {          // Map.cc:455
+            if (!in_board) {
                 E.mv_state[f] = MV_OOB;
                 continue;
             }

@@ -564,6 +564,48 @@ class GridWorld(Environment):
         """uniform random actions generated on the device (throughput runs only)"""
         self._lib.magent_b200_random_actions(self.game, self._hv(handle), None, int(seed))
 
+    def get_action_mask(self, handle):
+        """bool (n, n_action): which actions of every agent of the group would succeed if taken alone on the state as it
+        is now (include/magent_b200_ext.h magent_b200_get_action_mask has the definition).  Rows are in the order of
+        set_action; a dead, un-culled agent's row is all False.  The array is a cached receive buffer: valid until the
+        next call."""
+        g = self._hv(handle)
+        block = self._blocks.get((g, "mask"))
+        if block is None:
+            block = self._blocks[(g, "mask")] = _HostBlock(self._lib)
+        buf = block.view((self.get_num(handle), self.action_space[g][0]), np.uint8)
+        self._check(self._lib.magent_b200_get_action_mask(self.game, g, buf.ctypes.data), "get_action_mask")
+        return buf.view(np.bool_)
+
+    def get_action_mask_torch(self, handle, out=None):
+        """the legal-action mask (see get_action_mask) written straight into a CUDA torch.bool tensor (n, n_action):
+        logits.masked_fill_(~mask, -inf) before sampling.
+
+        out: a caller-owned contiguous CUDA tensor (rows, n_action), torch.bool or torch.uint8, with at least
+        get_num_bound(handle) rows; needed to record the call into a CUDA graph (capture_graph), since the call then
+        allocates nothing.  Returns the first get_num(handle) rows as torch.bool."""
+        import torch
+        g = self._hv(handle)
+        na = self.action_space[g][0]
+        n = self.get_num(handle)
+        if out is None:
+            out = torch.empty((n, na), dtype=torch.uint8, device="cuda")
+        else:
+            if not isinstance(out, torch.Tensor) or not out.is_cuda or out.dtype not in (torch.bool, torch.uint8):
+                raise ValueError("out must be a CUDA tensor of dtype torch.bool or torch.uint8")
+            if out.dim() != 2 or out.shape[1] != na or not out.is_contiguous() or out.shape[0] < self.get_num_bound(handle):
+                raise ValueError("out must be contiguous, of shape (rows, %d) with at least %d rows"
+                                 % (na, self.get_num_bound(handle)))
+        self._check(self._lib.magent_b200_get_action_mask(self.game, g, ctypes.c_void_p(out.data_ptr())),
+                    "get_action_mask")
+        return out.view(torch.bool)[:n]
+
+    def set_random_legal_actions(self, handle, seed):
+        """set_action with an action drawn uniformly from every agent's legal actions (get_action_mask), on the device:
+        the exploration baseline, and a much denser fight than set_random_actions produces"""
+        self._check(self._lib.magent_b200_random_legal_actions(self.game, self._hv(handle), int(seed)),
+                    "random_legal_actions")
+
     def get_counters(self):
         """int64 event counters accumulated on the device since construction"""
         buf = (ctypes.c_longlong * 16)()
