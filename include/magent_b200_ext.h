@@ -49,6 +49,24 @@ int magent_b200_get_action_mask(EnvHandle game, GroupHandle group, unsigned char
  * magent_b200_random_actions: the call counter of both calls and the device step counter ride in the seed, so a replayed
  * graph draws fresh actions.  Not part of parity.  Returns -1 for a bad group handle. */
 int magent_b200_random_legal_actions(EnvHandle game, GroupHandle group, unsigned long long seed);
+/* mean neighbour action (mean-field Q-learning / actor-critic): for every agent i of `group`, in ABI order (the rows of
+ * env_set_action, arenas concatenated), the mean one-hot action of its neighbours of group `of` (`of` == `group` is
+ * allowed).  The neighbours N(i) are the distinct agents j != i of `of`, in i's arena, whose presence i's own view shows:
+ * some in-range cell of i's view window (turn_mode: laid out in i's frame, as env_get_observation does) is a map cell
+ * that j's body covers.  A body larger than 1 x 1 counts once however many of its cells are in view.
+ *   count[i]   = |N(i)|                                                             int32 [n], may be NULL
+ *   mean[i][k] = (float)#{j in N(i): act_j == k} / (float)count[i], k < n_action(of)   float32 [n][n_action(of)]
+ * with IEEE round-to-nearest division.  act_j is the action j holds now: the one set_action / random_actions /
+ * random_legal_actions last gave it, which is the one the last env_step executed until the next set.  So called after
+ * env_step and before the next set_action it gives the previous step's mean action (what mean-field methods condition on);
+ * called after set_action it gives the actions just set.  A neighbour whose action is outside [0, n_action(of)) (added
+ * since the last step, or an id the step ignores) is counted in count and in no bin: its row sums to less than 1.  A row
+ * without neighbours is all zero; a dead, un-culled agent has an all-zero row and count 0.  Returns -1 for a bad `group`
+ * or `of` handle, or when one pointer is host memory and the other a CUDA device pointer.  Both host pointers: the call
+ * waits for the counts.  Both CUDA device pointers: no synchronisation, no allocation, recordable into a CUDA graph; rows
+ * are sized by the device-side counts, at most "num_bound" of them are written.  magent_b200_select_arena does not
+ * apply. */
+int magent_b200_get_mean_action(EnvHandle game, GroupHandle group, GroupHandle of, float *mean, int *count);
 /* compact observation hand-off (SURVEY.md 8f rank 2): same call, layout and pointer rules as env_get_observation
  * (reference src/runtime_api.h:35), but every element is an IEEE binary16 = the float32 value rounded to
  * nearest-even.  buffer[0] = view [n][view_h][view_w][n_channel], buffer[1] = feature [n][feature_size];

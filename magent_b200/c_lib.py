@@ -65,6 +65,7 @@ EXT_SIGNATURES = {
     "magent_b200_random_actions": ([_vp, ctypes.c_int, _vp, ctypes.c_ulonglong], ctypes.c_int),
     "magent_b200_get_action_mask": ([_vp, ctypes.c_int, _vp], ctypes.c_int),
     "magent_b200_random_legal_actions": ([_vp, ctypes.c_int, ctypes.c_ulonglong], ctypes.c_int),
+    "magent_b200_get_mean_action": ([_vp, ctypes.c_int, ctypes.c_int, _vp, _vp], ctypes.c_int),
     "magent_b200_get_observation_f16": ([_vp, ctypes.c_int, ctypes.POINTER(_vp)], ctypes.c_int),
     "magent_b200_get_global_state": ([_vp, _vp, ctypes.c_int], ctypes.c_int),
     "magent_b200_snapshot_arenas": ([_vp], ctypes.c_int),

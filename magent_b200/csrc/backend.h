@@ -80,6 +80,11 @@ __attribute__((weak)) void launch_action_mask(Ctx *, const EngineDev *dE, const 
                                               unsigned char *out, int n_total);
 __attribute__((weak)) void launch_random_legal_actions(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask,
                                                        int group, unsigned long long seed, int n_total);
+// Mean neighbour action of every agent of `group` over its neighbours of group `of` (nbr_phases.h): float
+// [n][n_action(of)] into `mean` and, unless null, int [n] into `count`, both device buffers.  n_total is the host's count,
+// an upper bound: the device-side offsets decide.  Weak like launch_action_mask: the engine refuses the call without it.
+__attribute__((weak)) void launch_mean_action(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group,
+                                              int of, float *mean, int *count, int n_total);
 // clear_dead: asynchronous read-back of the [G][A+1] offset table (launch_offsets) into page-locked memory
 void counts_fetch_begin(Ctx *, const int *dev_off, size_t n_ints);
 const int *counts_fetch_wait(Ctx *);     // blocks until the fetch has landed; valid until the next counts_fetch_begin

@@ -28,6 +28,7 @@ namespace mg { __device__ long long mg_phase_clock[8 * 32]; }
 #endif
 #include "obs_phases.h"
 #include "mask_phases.h"
+#include "nbr_phases.h"
 
 namespace cg = cooperative_groups;
 
@@ -46,7 +47,7 @@ static std::atomic<long long> g_launches{0};       // instrumentation only (mage
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize belongs to (function, device), not to an engine: it is only ever raised,
 // under a lock, so that a second engine with a smaller need cannot pull it from under the first
-enum { ATTR_STEP = 0, ATTR_OBS0 = 1, ATTR_N = 1 + 12, ATTR_MAX_DEVICES = 64 };
+enum { ATTR_STEP = 0, ATTR_OBS0 = 1, ATTR_MEAN = 1 + 12, ATTR_N, ATTR_MAX_DEVICES = 64 };
 static std::mutex g_attr_mu;
 static size_t g_attr_smem[ATTR_MAX_DEVICES][ATTR_N];
 template <class K>
@@ -840,6 +841,122 @@ void launch_random_legal_actions(Ctx *c, const EngineDev *dE, const EngineDev &h
     const int cpa = mask_chunks_per_arena(hE, group);
     random_legal_actions_kernel<<<(unsigned)((size_t)hE.A * cpa), MASK_THREADS, 0, c->stream>>>(dE, curmask, group, seed, n_total, cpa);
     post_launch("random_legal_actions_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
+// mean neighbour action (magent_b200_get_mean_action): nbr_phases.h for every observer of a group.  CTAs are dealt per
+// arena like action_mask_kernel (blockIdx says which arena, the device-side offsets decide how many observers it has,
+// the host's count is only an upper bound).  A CTA owns MEAN_OBS consecutive observers; warp w takes observers w, w + 8,
+// ... of them, one at a time, after its lanes have loaded all of their own fields at once.  The lanes stride over the
+// observer's in-range view cells through the CTA's view LUT (four in turn_mode, one per heading), and every lane issues
+// the `kind`-byte loads of MEAN_UNROLL cells before it looks at any of them, so the cell loads of an observer do not
+// wait on one another.  Only a cell whose byte shows group `of` (about 5 % of battle's cells) goes on to `occ`, the
+// footprint test of longer bodies and the neighbour's action; the counts land in the warp's shared-memory histogram of
+// n_action(of) ints.  The pad of the planes covers every view window in every heading: no bounds check on the bytes.
+constexpr int MEAN_THREADS = 256, MEAN_OBS = 128, MEAN_UNROLL = 4;
+constexpr int MEAN_WARPS = MEAN_THREADS / 32;
+static_assert(MEAN_OBS / MEAN_WARPS <= 32, "a warp's observers are loaded one per lane");
+// The kernel is latency-bound (a kind -> occ -> act chain per observer), so resident warps matter: five CTAs per SM
+// leave it 44 registers without spills (58 unbounded, four CTAs; six CTAs spill).  DESIGN.md §5 has the numbers.
+
+__global__ void __launch_bounds__(MEAN_THREADS, 5) mean_action_kernel(const EngineDev *gE, unsigned curmask, int g, int of,
+                                                                  float *mean, int *count, int n_total,
+                                                                  int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    __shared__ int n_in_s;
+    extern __shared__ __align__(16) unsigned char mean_smem[];
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int a = blockIdx.x / chunks_per_arena;
+    const int c0 = (blockIdx.x - a * chunks_per_arena) * MEAN_OBS;
+    const int *off = E.off + (size_t)g * (E.A + 1);
+    const int o0 = off[a];
+    int cta_cnt = min(MEAN_OBS, off[a + 1] - o0 - c0);
+    cta_cnt = min(cta_cnt, n_total - (o0 + c0));                 // never beyond the caller's buffers
+    if (cta_cnt <= 0) return;
+    const GroupDev &G = E.grp[g];
+    const int na = E.grp[of].n_action;
+    const int lut_stride = G.view_count;
+    // lut[k] = {offset of the map cell in the padded planes from the observer's own cell, dx | dy << 16}
+    int2 *lut = (int2 *)mean_smem;
+    int *hist = (int *)(lut + (E.turn_mode ? 4 : 1) * lut_stride) + warp * na;
+    if (warp == 0) {                                          // compact the view mask, order-preserving
+        const int cells = G.view_w * G.view_h;
+        int k = 0;
+        for (int base = 0; base < cells; base += 32) {
+            const int cell = base + lane;
+            const bool in = cell < cells && G.view_mask[cell];
+            const unsigned bal = __ballot_sync(0xffffffffu, in);
+            if (in) {
+                const int vy = cell / G.view_w, vx = cell - vy * G.view_w;
+                const int q = k + __popc(bal & ((1u << lane) - 1u));
+                for (int d = 0; d < (E.turn_mode ? 4 : 1); ++d) {
+                    int dx, dy;
+                    nbr_view_delta(E, G, d, vx, vy, dx, dy);
+                    lut[d * lut_stride + q] = make_int2(dy * E.kw + dx, (dx & 0xffff) | (int)((unsigned)dy << 16));
+                }
+            }
+            k += __popc(bal);
+        }
+        if (lane == 0) n_in_s = k;
+    }
+    __syncthreads();
+    const int n_in = n_in_s;
+    const int n_mine = cta_cnt > warp ? (cta_cnt - warp + MEAN_WARPS - 1) / MEAN_WARPS : 0;
+    NbrObserver mine;                                         // lane u: observer c0 + warp + MEAN_WARPS * u
+    mine.x = mine.y = 0; mine.dir = DIR_NORTH; mine.code = 0; mine.flags = FLAG_DEAD;
+    if (lane < n_mine) mine = nbr_observer(E, curmask, a, g, c0 + warp + MEAN_WARPS * lane);
+    const unsigned char *kplane = E.kind + (long)a * E.kplane;
+    for (int u = 0; u < n_mine; ++u) {
+        const int i = c0 + warp + MEAN_WARPS * u;
+        NbrObserver o;
+        o.x = __shfl_sync(0xffffffffu, mine.x, u); o.y = __shfl_sync(0xffffffffu, mine.y, u);
+        o.dir = __shfl_sync(0xffffffffu, mine.dir, u); o.code = code_make(g, i);
+        o.flags = (unsigned char)__shfl_sync(0xffffffffu, (int)mine.flags, u);
+        for (int k = lane; k < na; k += 32) hist[k] = 0;
+        __syncwarp();
+        int cnt = 0;
+        if (!(o.flags & FLAG_DEAD)) {
+            const unsigned char *kp = kplane + (long)(o.y + E.kpad) * E.kw + o.x + E.kpad;
+            const int2 *l = lut + (E.turn_mode ? o.dir * lut_stride : 0);
+            for (int q0 = lane; q0 < n_in; q0 += 32 * MEAN_UNROLL) {
+                int t[MEAN_UNROLL];
+#pragma unroll
+                for (int r = 0; r < MEAN_UNROLL; ++r) t[r] = q0 + 32 * r < n_in ? __ldg(kp + l[q0 + 32 * r].x) : 0;
+#pragma unroll
+                for (int r = 0; r < MEAN_UNROLL; ++r) {
+                    if (!nbr_kind_of(t[r], of)) continue;
+                    const int d = l[q0 + 32 * r].y;
+                    const int j = nbr_at(E, curmask, a, g, of, o, o.x + (short)(d & 0xffff), o.y + (d >> 16));
+                    if (j < 0) continue;
+                    ++cnt;
+                    const int k = nbr_bin(E, curmask, a, of, j);
+                    if (k >= 0) atomicAdd(hist + k, 1);
+                }
+            }
+            cnt = __reduce_add_sync(0xffffffffu, cnt);
+        }
+        __syncwarp();
+        float *row = mean + (size_t)(o0 + i) * na;
+        for (int k = lane; k < na; k += 32) row[k] = nbr_mean(hist[k], cnt);
+        if (count && lane == 0) count[o0 + i] = cnt;
+        __syncwarp();                                         // the histogram is read before the next observer clears it
+    }
+}
+
+void launch_mean_action(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group, int of,
+                        float *mean, int *count, int n_total) {
+    DeviceGuard guard(c);
+    const size_t smem = (size_t)(hE.turn_mode ? 4 : 1) * hE.grp[group].view_count * sizeof(int2) +
+                        (size_t)MEAN_WARPS * hE.grp[of].n_action * sizeof(int);
+    if (smem + sizeof(EngineDev) + 64 > 227 * 1024)
+        mg::fatal("mean action: a view of %d cells is more than the kernel holds", hE.grp[group].view_count);
+    if (smem + sizeof(EngineDev) + 64 > 48 * 1024) ensure_dynamic_smem(c->device, ATTR_MEAN, mean_action_kernel, smem);
+    const int cpa = (hE.grp[group].cap + MEAN_OBS - 1) / MEAN_OBS;
+    mean_action_kernel<<<(unsigned)((size_t)hE.A * cpa), MEAN_THREADS, smem, c->stream>>>(dE, curmask, group, of, mean,
+                                                                                          count, n_total, cpa);
+    post_launch("mean_action_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------

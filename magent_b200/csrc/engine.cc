@@ -1243,6 +1243,31 @@ int Engine::random_legal_actions(int group, unsigned long long seed) {
     return 0;
 }
 
+// Mean neighbour action of one group over the agents of group `of` it sees.  Same pointer discipline as
+// get_action_mask: device buffers take one kernel clamped by the device-side counts, host buffers settle the counts and go
+// through the i/o staging (mean and count share one staging block).
+int Engine::get_mean_action(int group, int of, float *mean, int *count) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_mean_action", group);
+    if (of < 0 || of >= G()) return refuse("invalid group handle %d for `of` in get_mean_action", of);
+    if (!be::launch_mean_action) return refuse("the %s backend has no mean-action kernel", be::name());
+    const bool dev = mean && be::is_device_ptr(mean);
+    if (mean && count && be::is_device_ptr(count) != dev)
+        return refuse("get_mean_action: mean and count must both be host memory or both CUDA device memory");
+    to_device();
+    if (!dev) settle_counts();
+    const int n = total(group);
+    if (n == 0) return 0;
+    if (!mean) return refuse("get_mean_action needs a mean buffer");
+    if (dev) { be::launch_mean_action(bx_, dE_, hE_, curmask_, group, of, mean, count, n); return 0; }
+    const size_t mean_bytes = (size_t)n * group_type_[of]->n_action * 4, count_bytes = count ? (size_t)n * 4 : 0;
+    char *st = (char *)io_stage(mean_bytes + count_bytes);
+    be::launch_mean_action(bx_, dE_, hE_, curmask_, group, of, (float *)st, count ? (int *)(st + mean_bytes) : nullptr, n);
+    be::d2h(bx_, mean, st, mean_bytes);
+    if (count) be::d2h(bx_, count, st + mean_bytes, count_bytes);
+    io_[IO_D2H] += (long long)(mean_bytes + count_bytes);
+    return 0;
+}
+
 void Engine::step(int *done) {                                        // GridWorld.cc:456-631
     to_device();
     StepArgs S;

@@ -123,6 +123,9 @@ public:
     // -1 and the last error when refused.
     int get_action_mask(int group, unsigned char *buf);
     int random_legal_actions(int group, unsigned long long seed);
+    // mean neighbour action (nbr_phases.h): float [n][n_action(of)] and int [n] (count may be null) of one group.
+    // -1 and the last error when refused.
+    int get_mean_action(int group, int of, float *mean, int *count);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads

@@ -107,6 +107,9 @@ MG_API int magent_b200_get_action_mask(EnvHandle game, GroupHandle group, unsign
 MG_API int magent_b200_random_legal_actions(EnvHandle game, GroupHandle group, unsigned long long seed) {
     return E(game)->random_legal_actions(group, seed);
 }
+MG_API int magent_b200_get_mean_action(EnvHandle game, GroupHandle group, GroupHandle of, float *mean, int *count) {
+    return E(game)->get_mean_action(group, of, mean, count);
+}
 MG_API int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **buffer) {
     E(game)->get_observation(group, buffer, 1);
     return 0;

@@ -606,6 +606,55 @@ class GridWorld(Environment):
         self._check(self._lib.magent_b200_random_legal_actions(self.game, self._hv(handle), int(seed)),
                     "random_legal_actions")
 
+    def get_mean_action(self, handle, of=None):
+        """(mean float32 (n, n_action(of)), count int32 (n,)): for every agent of the group, the mean one-hot action of
+        the agents of group `of` (default: its own group) that its view shows, and how many those are -- mean-field
+        Q-learning's neighbour action (include/magent_b200_ext.h magent_b200_get_mean_action has the definition).  Called
+        after step and before the next set_action it gives the previous step's actions.  Rows are in the order of
+        set_action.  Both arrays are cached receive buffers: valid until the next call."""
+        g = self._hv(handle)
+        o = g if of is None else self._hv(of)
+        n = self.get_num(handle)
+        block = self._blocks.get((g, "mean"))
+        if block is None:
+            block = self._blocks[(g, "mean")] = _HostBlock(self._lib)
+        na = self.action_space[o][0]
+        raw = block.view((n * (na + 1),), np.float32)
+        mean, count = raw[:n * na].reshape(n, na), raw[n * na:].view(np.int32)
+        self._check(self._lib.magent_b200_get_mean_action(self.game, g, o, mean.ctypes.data, count.ctypes.data),
+                    "get_mean_action")
+        return mean, count
+
+    def get_mean_action_torch(self, handle, of=None, out=None):
+        """the mean neighbour action (see get_mean_action) written straight into CUDA tensors: returns (mean float32
+        (n, n_action(of)), count int32 (n,)).
+
+        out: a caller-owned pair (mean, count) of contiguous CUDA tensors, float32 (rows, n_action(of)) and int32
+        (rows,), with at least get_num_bound(handle) rows each; needed to record the call into a CUDA graph
+        (capture_graph), since the call then allocates nothing.  Returns the first get_num(handle) rows of each."""
+        import torch
+        g = self._hv(handle)
+        o = g if of is None else self._hv(of)
+        na = self.action_space[o][0]
+        n = self.get_num(handle)
+        if out is None:
+            mean = torch.empty((n, na), dtype=torch.float32, device="cuda")
+            count = torch.empty((n,), dtype=torch.int32, device="cuda")
+        else:
+            if not isinstance(out, (tuple, list)) or len(out) != 2:
+                raise ValueError("out must be a (mean, count) pair of CUDA tensors")
+            mean, count = out
+            bound = self.get_num_bound(handle)
+            for t, dt, nd in ((mean, torch.float32, 2), (count, torch.int32, 1)):
+                if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dt:
+                    raise ValueError("out must be a CUDA float32 mean tensor and a CUDA int32 count tensor")
+                if t.dim() != nd or not t.is_contiguous() or t.shape[0] < bound or (nd == 2 and t.shape[1] != na):
+                    raise ValueError("out must be contiguous, of shapes (rows, %d) and (rows,) with at least %d rows"
+                                     % (na, bound))
+        self._check(self._lib.magent_b200_get_mean_action(self.game, g, o, ctypes.c_void_p(mean.data_ptr()),
+                                                          ctypes.c_void_p(count.data_ptr())), "get_mean_action")
+        return mean[:n], count[:n]
+
     def get_counters(self):
         """int64 event counters accumulated on the device since construction"""
         buf = (ctypes.c_longlong * 16)()
