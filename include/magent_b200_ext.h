@@ -67,6 +67,28 @@ int magent_b200_random_legal_actions(EnvHandle game, GroupHandle group, unsigned
  * are sized by the device-side counts, at most "num_bound" of them are written.  magent_b200_select_arena does not
  * apply. */
 int magent_b200_get_mean_action(EnvHandle game, GroupHandle group, GroupHandle of, float *mean, int *count);
+/* nearest visible neighbours (graph-convolutional and attention policies): for every agent i of `group`, in ABI order,
+ * the first k of its neighbours N(i) in group `of`, nearest first.  N(i) is exactly the neighbour set of
+ * magent_b200_get_mean_action (`of` == `group` allowed).  Every view cell (vx, vy) of i's window (turn_mode: laid out in
+ * i's frame) has the key (d2, vy * view_w + vx), compared in that order: d2 is the squared Euclidean distance, in map
+ * cells, from the map cell it shows to i's footprint [x, x + bw) x [y, y + bh) (body dimensions rotated by i's heading;
+ * 0 on the footprint itself).  The distance is to the body, not to the window centre, because sector views do not centre
+ * the window on the observer.  A neighbour's key is the smallest key among the in-range, on-board cells of i's window that
+ * its body covers (a body larger than 1 x 1 appears once, at its nearest visible cell).  Neighbours are ordered by key
+ * and the first min(k, |N(i)|) are written:
+ *   idx[i][r]    = j's row in group `of`'s ABI concatenation now (its arena's offset + its index): its row in
+ *                  get_observation(of), get_pos(of) and any per-agent tensor kept in that order     int32 [n][k]
+ *   rel[i][r][:] = (vy, vx), the view cell where that nearest visible cell lies: where i's own observation shows j
+ *                                                                                 int32 [n][k][2], may be NULL
+ *   count[i]     = |N(i)|, not capped by k (= get_mean_action's count)            int32 [n], may be NULL
+ * Unused slots hold -1 (rel: (-1, -1)).  A dead, un-culled observer has an all -1 row and count 0; dead neighbours have
+ * left the map.  The indices go stale with the next clear_dead, restore_arenas or add_agents, like every row-ordered
+ * output.  1 <= k <= 32.  Returns -1, sets magent_b200_last_error and writes nothing for a bad `group` or `of` handle, k
+ * out of range, a NULL idx, pointers that mix host and CUDA device memory, or a backend without the kernel.  Host
+ * pointers: the call waits for the counts.  CUDA device pointers: no synchronisation, no allocation, recordable into a
+ * CUDA graph; rows are sized by the device-side counts, at most "num_bound" of them are written.
+ * magent_b200_select_arena does not apply. */
+int magent_b200_get_neighbours(EnvHandle game, GroupHandle group, GroupHandle of, int k, int *idx, int *rel, int *count);
 /* compact observation hand-off (SURVEY.md 8f rank 2): same call, layout and pointer rules as env_get_observation
  * (reference src/runtime_api.h:35), but every element is an IEEE binary16 = the float32 value rounded to
  * nearest-even.  buffer[0] = view [n][view_h][view_w][n_channel], buffer[1] = feature [n][feature_size];

@@ -85,6 +85,14 @@ __attribute__((weak)) void launch_random_legal_actions(Ctx *, const EngineDev *d
 // an upper bound: the device-side offsets decide.  Weak like launch_action_mask: the engine refuses the call without it.
 __attribute__((weak)) void launch_mean_action(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group,
                                               int of, float *mean, int *count, int n_total);
+// The first k (1..32) neighbours of group `of`, nearest first (nbr_phases.h nbr_cell_key), of every agent of `group`: int
+// [n][k] rows of `of` into `idx`, unless null int [n][k][2] (vy, vx) into `rel` and int [n] |N(i)| into `count`, all
+// device buffers; unused slots -1.  `lut` is the group's view LUT in key order (struct NbrCell, one run of view_count
+// entries per heading in turn_mode), a device buffer.  n_total is the host's count, an upper bound: the device-side
+// offsets decide.  Weak like launch_mean_action: the engine refuses the call without it.
+__attribute__((weak)) void launch_neighbours(Ctx *, const EngineDev *dE, const EngineDev &hE, const NbrCell *lut,
+                                             unsigned curmask, int group, int of, int k, int *idx, int *rel, int *count,
+                                             int n_total);
 // clear_dead: asynchronous read-back of the [G][A+1] offset table (launch_offsets) into page-locked memory
 void counts_fetch_begin(Ctx *, const int *dev_off, size_t n_ints);
 const int *counts_fetch_wait(Ctx *);     // blocks until the fetch has landed; valid until the next counts_fetch_begin

@@ -960,6 +960,95 @@ void launch_mean_action(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsign
 }
 
 // ------------------------------------------------------------------------------------------------
+// nearest visible neighbours (magent_b200_get_neighbours): the first k members of N(i) in key order (nbr_phases.h
+// nbr_cell_key) for every observer of a group.  The mapping is mean_action_kernel's: CTAs are dealt per arena, a CTA
+// owns NBR_OBS consecutive observers, warp w takes observers w, w + 8, ... of them one at a time after its lanes have
+// loaded all of their fields.  The lanes walk the group's view LUT, sorted by key on the host (Engine::to_device), in
+// rounds of 32 cells: lane order is key order, so a ballot over the cells that list a neighbour hands out consecutive
+// slots (found so far + popc of the lower lanes) and the row comes out sorted without a sort.  Every lane issues the
+// `kind`-byte loads of NBR_ROUNDS rounds before it looks at any of them; only a byte that shows group `of` goes on to
+// `occ` and, for a longer body, the smallest-key test (nbr_nearest_at).  Without `count` the warp stops after the round
+// that fills slot k.  The LUT stays in global memory (L1-resident: 16 bytes per cell, the same for every observer), so the
+// CTA holds nothing but the EngineDev copy.
+constexpr int NBR_THREADS = 256, NBR_OBS = 128, NBR_ROUNDS = 4;
+constexpr int NBR_WARPS = NBR_THREADS / 32;
+static_assert(NBR_OBS / NBR_WARPS <= 32, "a warp's observers are loaded one per lane");
+
+__global__ void __launch_bounds__(NBR_THREADS, 5) neighbours_kernel(const EngineDev *gE, const NbrCell *lut,
+                                                                    unsigned curmask, int g, int of, int k, int *idx,
+                                                                    int *rel, int *count, int n_total,
+                                                                    int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int a = blockIdx.x / chunks_per_arena;
+    const int c0 = (blockIdx.x - a * chunks_per_arena) * NBR_OBS;
+    const int o0 = E.off[(size_t)g * (E.A + 1) + a];
+    int cta_cnt = min(NBR_OBS, E.off[(size_t)g * (E.A + 1) + a + 1] - o0 - c0);
+    cta_cnt = min(cta_cnt, n_total - (o0 + c0));                 // never beyond the caller's buffers
+    if (cta_cnt <= 0) return;
+    const int base = E.off[(size_t)of * (E.A + 1) + a];          // row of j = base + j in `of`'s concatenation
+    const int n_in = E.grp[g].view_count;
+    const int n_mine = cta_cnt > warp ? (cta_cnt - warp + NBR_WARPS - 1) / NBR_WARPS : 0;
+    NbrObserver mine;                                             // lane u: observer c0 + warp + NBR_WARPS * u
+    mine.x = mine.y = 0; mine.dir = DIR_NORTH; mine.code = 0; mine.flags = FLAG_DEAD;
+    if (lane < n_mine) mine = nbr_observer(E, curmask, a, g, c0 + warp + NBR_WARPS * lane);
+    const unsigned char *kplane = E.kind + (long)a * E.kplane;
+    const unsigned lower = (1u << lane) - 1u;
+    for (int u = 0; u < n_mine; ++u) {
+        const int i = c0 + warp + NBR_WARPS * u;
+        NbrObserver o;
+        o.x = __shfl_sync(0xffffffffu, mine.x, u); o.y = __shfl_sync(0xffffffffu, mine.y, u);
+        o.dir = __shfl_sync(0xffffffffu, mine.dir, u); o.code = code_make(g, i);
+        o.flags = (unsigned char)__shfl_sync(0xffffffffu, (int)mine.flags, u);
+        const size_t row = (size_t)(o0 + i) * k;
+        int found = 0;
+        if (!(o.flags & FLAG_DEAD)) {
+            const unsigned char *kp = kplane + (long)(o.y + E.kpad) * E.kw + o.x + E.kpad;
+            const NbrCell *l = lut + (E.turn_mode ? o.dir * n_in : 0);
+            // warp-uniform bounds: every lane takes part in every ballot
+            for (int q0 = lane; q0 - lane < n_in && (count || found < k); q0 += 32 * NBR_ROUNDS) {
+                int t[NBR_ROUNDS];
+#pragma unroll
+                for (int r = 0; r < NBR_ROUNDS; ++r) t[r] = q0 + 32 * r < n_in ? __ldg(kp + __ldg(&l[q0 + 32 * r].off)) : 0;
+#pragma unroll
+                for (int r = 0; r < NBR_ROUNDS; ++r) {
+                    if (!count && found >= k) break;
+                    int j = -1, cell = 0;
+                    if (nbr_kind_of(t[r], of)) {
+                        const int4 c = __ldg((const int4 *)(l + q0 + 32 * r));
+                        j = nbr_nearest_at(E, curmask, a, g, of, o, o.x + (short)(c.y & 0xffff), o.y + (c.y >> 16), c.z);
+                        cell = c.w;
+                    }
+                    const unsigned hits = __ballot_sync(0xffffffffu, j >= 0);
+                    const int slot = found + __popc(hits & lower);
+                    if (j >= 0 && slot < k) {
+                        idx[row + slot] = base + j;
+                        if (rel) { rel[2 * (row + slot)] = cell >> 16; rel[2 * (row + slot) + 1] = cell & 0xffff; }
+                    }
+                    found += __popc(hits);
+                }
+            }
+        }
+        for (int s = found + lane; s < k; s += 32) {              // unused slots
+            idx[row + s] = -1;
+            if (rel) { rel[2 * (row + s)] = -1; rel[2 * (row + s) + 1] = -1; }
+        }
+        if (count && lane == 0) count[o0 + i] = found;
+    }
+}
+
+void launch_neighbours(Ctx *c, const EngineDev *dE, const EngineDev &hE, const NbrCell *lut, unsigned curmask, int group,
+                       int of, int k, int *idx, int *rel, int *count, int n_total) {
+    DeviceGuard guard(c);
+    const int cpa = (hE.grp[group].cap + NBR_OBS - 1) / NBR_OBS;
+    neighbours_kernel<<<(unsigned)((size_t)hE.A * cpa), NBR_THREADS, 0, c->stream>>>(dE, lut, curmask, group, of, k, idx,
+                                                                                    rel, count, n_total, cpa);
+    post_launch("neighbours_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
 // obs_prepare: the minimap of one observation state (GridWorld.cc:328-357): per (arena, group) the number of agents in
 // every coarse cell of the OBSERVER's view-sized grid, divided by the group's size.  Dead-but-unculled agents count,
 // absorbed ones do not when the observer's type can absorb (:343-347).  (The hp_norm plane the render also needs is

@@ -233,6 +233,13 @@ struct ObsArgs {
     int grid = 0, chunk = 0, tile = 0;
 };
 
+// One entry of a group's view LUT in the key order of magent_b200_get_neighbours (nbr_phases.h nbr_cell_key).
+// Engine::to_device builds it on the host, one run of view_count entries per heading in turn_mode, and keeps it outside
+// EngineDev: {offset of the map cell in the padded planes from the observer's own cell, dx | dy << 16, key, vx | vy << 16}.
+struct alignas(16) NbrCell {
+    int off, delta, key, cell;
+};
+
 enum InfoKind { INFO_ID = 0, INFO_POS, INFO_ALIVE, INFO_REWARD, INFO_ACTION_SCATTER, INFO_HP };
 
 }  // namespace mg

@@ -1,6 +1,7 @@
 // engine.cc -- host side of the B200 grid-world engine.  See engine.h.
 #include "engine.h"
 #include "step_phases.h"
+#include "nbr_phases.h"
 
 #include <math.h>
 #include <stdarg.h>
@@ -599,6 +600,8 @@ void Engine::free_device() {
     if (d_io_stage_) be::dfree(bx_, d_io_stage_);
     d_view_stage_ = d_feat_stage_ = nullptr; d_io_stage_ = nullptr;
     view_stage_bytes_ = feat_stage_bytes_ = io_stage_bytes_ = 0;
+    d_nbr_lut_ = nullptr;
+    nbr_lut_.clear();
     dE_ = nullptr;
     cap_.clear();
 }
@@ -640,6 +643,47 @@ static T *upload_vec(be::Ctx *bx_, std::vector<void *> &allocs, const std::vecto
     allocs.push_back(p);
     if (!v.empty()) be::h2d(bx_, p, v.data(), v.size() * sizeof(T));
     return p;
+}
+
+// The view LUTs of get_neighbours: per group and heading (one run of view_count cells, four in turn_mode) the in-range
+// cells of the window in key order, built from the group's geometry alone with the functions the kernel and the test
+// emulation use (nbr_phases.h).  Uploaded when the device image is new or the LUTs changed (turn_mode or the padded plane
+// width), so the call itself never allocates or copies.
+void Engine::upload_nbr_luts(bool force) {
+    const int Gn = G();
+    std::vector<NbrCell> lut;
+    nbr_lut_base_.assign(Gn, 0);
+    nbr_key_fits_.assign(Gn, 0);
+    for (int g = 0; g < Gn; ++g) {
+        const AgentTypeDef &t = *group_type_[g];
+        const GroupDev &D = hE_.grp[g];
+        nbr_lut_base_[g] = lut.size();
+        // no in-range cell lies farther than kpad cells from the body on either axis: d2 <= 2 kpad^2
+        const long long cells = (long long)t.view.width * t.view.height;
+        if ((2LL * hE_.kpad * hE_.kpad + 1) * cells > 0x7fffffffLL) continue;
+        nbr_key_fits_[g] = 1;
+        for (int d = 0; d < (turn_mode_ ? 4 : 1); ++d) {
+            const int dir = turn_mode_ ? d : DIR_NORTH;
+            const size_t first = lut.size();
+            for (int vy = 0; vy < t.view.height; ++vy)
+                for (int vx = 0; vx < t.view.width; ++vx) {
+                    if (!t.view.mask[(size_t)vy * t.view.width + vx]) continue;
+                    int dx, dy;
+                    nbr_view_delta(hE_, D, dir, vx, vy, dx, dy);
+                    NbrCell c;
+                    c.off = dy * hE_.kw + dx;
+                    c.delta = (dx & 0xffff) | (int)((unsigned)dy << 16);
+                    c.key = nbr_cell_key(D, dir, dx, dy, vx, vy);
+                    c.cell = vx | vy << 16;
+                    lut.push_back(c);
+                }
+            std::sort(lut.begin() + first, lut.end(), [](const NbrCell &p, const NbrCell &q) { return p.key < q.key; });
+        }
+    }
+    const bool same = lut.size() == nbr_lut_.size() && (lut.empty() || !memcmp(lut.data(), nbr_lut_.data(), lut.size() * sizeof(NbrCell)));
+    if (!force && same) return;
+    if (!lut.empty()) be::h2d(bx_, d_nbr_lut_, lut.data(), lut.size() * sizeof(NbrCell));
+    nbr_lut_.swap(lut);
 }
 
 void Engine::to_device() {
@@ -737,6 +781,9 @@ void Engine::to_device() {
         hE_.mm_total = (int *)dalloc((size_t)A_ * Gn * 4);
         d_mm_val_ = (float *)dalloc((size_t)A_ * Gn * max_cells * 4);
         hE_.rules = (const RuleDev *)dalloc(sizeof(RuleDev) * (compiled_rules_.size() + 1));
+        size_t lut_cells = 0;                         // room for four headings: turn_mode may change without a re-allocation
+        for (int g = 0; g < Gn; ++g) lut_cells += 4 * (size_t)hE_.grp[g].view_count;
+        d_nbr_lut_ = (NbrCell *)dalloc(sizeof(NbrCell) * lut_cells);
         dE_ = (EngineDev *)dalloc(sizeof(EngineDev));
     }
     // constants that may change between episodes without a re-allocation
@@ -775,6 +822,7 @@ void Engine::to_device() {
     }
     for (int g = 0; g < Gn; ++g) hE_.grp[g].feature_size = feature_size(g);
     curmask_ = 0;
+    upload_nbr_luts(realloc);
 
     // ---- pack and upload the state
     std::vector<int> ibuf; std::vector<float> fbuf; std::vector<unsigned char> bbuf;
@@ -1265,6 +1313,37 @@ int Engine::get_mean_action(int group, int of, float *mean, int *count) {
     be::d2h(bx_, mean, st, mean_bytes);
     if (count) be::d2h(bx_, count, st + mean_bytes, count_bytes);
     io_[IO_D2H] += (long long)(mean_bytes + count_bytes);
+    return 0;
+}
+
+// The first k neighbours of one group in group `of`, nearest first.  Same pointer discipline as get_mean_action: device
+// buffers take one kernel clamped by the device-side counts, host buffers settle the counts and go through the i/o
+// staging (idx, rel and count share one staging block).
+int Engine::get_neighbours(int group, int of, int k, int *idx, int *rel, int *count) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_neighbours", group);
+    if (of < 0 || of >= G()) return refuse("invalid group handle %d for `of` in get_neighbours", of);
+    if (k < 1 || k > 32) return refuse("get_neighbours: k = %d is outside [1, 32]", k);
+    if (!idx) return refuse("get_neighbours needs an idx buffer");
+    if (!be::launch_neighbours) return refuse("the %s backend has no neighbours kernel", be::name());
+    const bool dev = be::is_device_ptr(idx);
+    if ((rel && be::is_device_ptr(rel) != dev) || (count && be::is_device_ptr(count) != dev))
+        return refuse("get_neighbours: idx, rel and count must all be host memory or all CUDA device memory");
+    to_device();
+    if (!nbr_key_fits_[group])
+        return refuse("get_neighbours: the view of group %d is too large to order its cells by an int key", group);
+    if (!dev) settle_counts();
+    const int n = total(group);
+    if (n == 0) return 0;
+    const NbrCell *lut = d_nbr_lut_ + nbr_lut_base_[group];
+    if (dev) { be::launch_neighbours(bx_, dE_, hE_, lut, curmask_, group, of, k, idx, rel, count, n); return 0; }
+    const size_t idx_bytes = (size_t)n * k * 4, rel_bytes = rel ? 2 * idx_bytes : 0, count_bytes = count ? (size_t)n * 4 : 0;
+    char *st = (char *)io_stage(idx_bytes + rel_bytes + count_bytes);
+    be::launch_neighbours(bx_, dE_, hE_, lut, curmask_, group, of, k, (int *)st, rel ? (int *)(st + idx_bytes) : nullptr,
+                          count ? (int *)(st + idx_bytes + rel_bytes) : nullptr, n);
+    be::d2h(bx_, idx, st, idx_bytes);
+    if (rel) be::d2h(bx_, rel, st + idx_bytes, rel_bytes);
+    if (count) be::d2h(bx_, count, st + idx_bytes + rel_bytes, count_bytes);
+    io_[IO_D2H] += (long long)(idx_bytes + rel_bytes + count_bytes);
     return 0;
 }
 

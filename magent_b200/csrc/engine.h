@@ -126,6 +126,9 @@ public:
     // mean neighbour action (nbr_phases.h): float [n][n_action(of)] and int [n] (count may be null) of one group.
     // -1 and the last error when refused.
     int get_mean_action(int group, int of, float *mean, int *count);
+    // the first k neighbours of group `of`, nearest first (nbr_phases.h nbr_cell_key): int [n][k] rows of `of`, int
+    // [n][k][2] view cells and int [n] neighbour counts (rel and count may be null).  -1 and the last error when refused.
+    int get_neighbours(int group, int of, int k, int *idx, int *rel, int *count);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads
@@ -181,6 +184,14 @@ private:
     std::vector<int> order_;            // groups with set_action this step, in call order
     void *d_view_stage_ = nullptr, *d_feat_stage_ = nullptr;
     float *d_mm_val_ = nullptr;
+    // the view LUTs of get_neighbours in key order, every group's and heading's runs in one device buffer (outside
+    // EngineDev, which seven kernels copy into shared memory): group g's start at nbr_lut_base_[g]; nbr_lut_ is the host
+    // copy last uploaded; nbr_key_fits_[g] == 0 when g's keys would not fit an int (the call is then refused)
+    NbrCell *d_nbr_lut_ = nullptr;
+    std::vector<NbrCell> nbr_lut_;
+    std::vector<size_t> nbr_lut_base_;
+    std::vector<unsigned char> nbr_key_fits_;
+    void upload_nbr_luts(bool force);
     size_t view_stage_bytes_ = 0, feat_stage_bytes_ = 0;
     void *d_io_stage_ = nullptr; size_t io_stage_bytes_ = 0;
     void *h_feat_stage_ = nullptr; size_t h_feat_stage_bytes_ = 0;      // page-locked staging of the feature rows (host path)

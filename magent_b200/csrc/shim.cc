@@ -110,6 +110,10 @@ MG_API int magent_b200_random_legal_actions(EnvHandle game, GroupHandle group, u
 MG_API int magent_b200_get_mean_action(EnvHandle game, GroupHandle group, GroupHandle of, float *mean, int *count) {
     return E(game)->get_mean_action(group, of, mean, count);
 }
+MG_API int magent_b200_get_neighbours(EnvHandle game, GroupHandle group, GroupHandle of, int k, int *idx, int *rel,
+                                      int *count) {
+    return E(game)->get_neighbours(group, of, k, idx, rel, count);
+}
 MG_API int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **buffer) {
     E(game)->get_observation(group, buffer, 1);
     return 0;

@@ -655,6 +655,68 @@ class GridWorld(Environment):
                                                           ctypes.c_void_p(count.data_ptr())), "get_mean_action")
         return mean[:n], count[:n]
 
+    def get_neighbours(self, handle, k, of=None):
+        """(idx int32 (n, k), rel int32 (n, k, 2), count int32 (n,)): for every agent of the group, the first k of the
+        agents of group `of` (default: its own group) that its view shows, nearest first -- the neighbour lists of
+        graph-convolutional and attention policies (include/magent_b200_ext.h magent_b200_get_neighbours has the
+        definition).  idx: their rows in group `of`'s order (get_pos(of), get_observation(of)), rel: the (vy, vx) view
+        cell where the observer's own observation shows them, count: how many neighbours it has in all.  Unused slots
+        are -1.  Rows are in the order of set_action.  The arrays are cached receive buffers: valid until the next call."""
+        g = self._hv(handle)
+        o = g if of is None else self._hv(of)
+        k = int(k)
+        if not 1 <= k <= 32:
+            raise ValueError("k must be in [1, 32], got %d" % k)
+        n = self.get_num(handle)
+        block = self._blocks.get((g, "nbr"))
+        if block is None:
+            block = self._blocks[(g, "nbr")] = _HostBlock(self._lib)
+        raw = block.view((n * (3 * k + 1),), np.int32)
+        idx, rel, count = raw[:n * k].reshape(n, k), raw[n * k:3 * n * k].reshape(n, k, 2), raw[3 * n * k:]
+        self._check(self._lib.magent_b200_get_neighbours(self.game, g, o, k, idx.ctypes.data, rel.ctypes.data,
+                                                         count.ctypes.data), "get_neighbours")
+        return idx, rel, count
+
+    def get_neighbours_torch(self, handle, k, of=None, out=None):
+        """the nearest visible neighbours (see get_neighbours) written straight into CUDA tensors: returns (idx int32
+        (n, k), rel int32 (n, k, 2), count int32 (n,)).
+
+        out: a caller-owned triple (idx, rel, count) of contiguous CUDA int32 tensors of shapes (rows, k), (rows, k, 2)
+        and (rows,), with at least get_num_bound(handle) rows each; needed to record the call into a CUDA graph
+        (capture_graph), since the call then allocates nothing.  rel and count may be None: they are then neither
+        computed nor written (without count the kernel stops at the k-th neighbour), and None comes back in their place.
+        Returns the first get_num(handle) rows of each."""
+        import torch
+        g = self._hv(handle)
+        o = g if of is None else self._hv(of)
+        k = int(k)
+        if not 1 <= k <= 32:
+            raise ValueError("k must be in [1, 32], got %d" % k)
+        n = self.get_num(handle)
+        if out is None:
+            idx = torch.empty((n, k), dtype=torch.int32, device="cuda")
+            rel = torch.empty((n, k, 2), dtype=torch.int32, device="cuda")
+            count = torch.empty((n,), dtype=torch.int32, device="cuda")
+        else:
+            if not isinstance(out, (tuple, list)) or len(out) != 3:
+                raise ValueError("out must be an (idx, rel, count) triple of CUDA tensors")
+            idx, rel, count = out
+            bound = self.get_num_bound(handle)
+            for t, shape, opt in ((idx, (k,), False), (rel, (k, 2), True), (count, (), True)):
+                if t is None and opt:
+                    continue
+                if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.int32:
+                    raise ValueError("out must hold CUDA int32 tensors (rel and count may be None)")
+                if t.dim() != 1 + len(shape) or not t.is_contiguous() or t.shape[0] < bound or tuple(t.shape[1:]) != shape:
+                    raise ValueError("out must be contiguous, of shapes (rows, %d), (rows, %d, 2) and (rows,) with at "
+                                     "least %d rows" % (k, k, bound))
+        if idx.shape[0] == 0:            # no row can be written (num_bound is 0), and an empty tensor's pointer is NULL
+            return idx, rel, count
+        ptr = (lambda t: None if t is None else ctypes.c_void_p(t.data_ptr()))
+        self._check(self._lib.magent_b200_get_neighbours(self.game, g, o, k, ptr(idx), ptr(rel), ptr(count)),
+                    "get_neighbours")
+        return idx[:n], None if rel is None else rel[:n], None if count is None else count[:n]
+
     def get_counters(self):
         """int64 event counters accumulated on the device since construction"""
         buf = (ctypes.c_longlong * 16)()
