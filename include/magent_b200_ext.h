@@ -89,6 +89,30 @@ int magent_b200_get_mean_action(EnvHandle game, GroupHandle group, GroupHandle o
  * CUDA graph; rows are sized by the device-side counts, at most "num_bound" of them are written.
  * magent_b200_select_arena does not apply. */
 int magent_b200_get_neighbours(EnvHandle game, GroupHandle group, GroupHandle of, int k, int *idx, int *rel, int *count);
+/* stable agent slots (rollout buffers, recurrent state, mixers: anything that needs one fixed index per agent for the
+ * whole episode, and fixed-shape CUDA-graph training steps).  Every row-ordered output keeps its row order; this call
+ * serves the two index maps between rows and slots.
+ *   The slot of an agent is the number of agents of its group that were placed into its arena before it since that
+ *   arena's last env_reset.  Placement is add_agents in any method, including mid-episode and through
+ *   magent_b200_select_arena.  So right after placement the slot equals the agent's index within its arena and group.  A
+ *   slot is never reused within an episode, and clear_dead keeps it.  A restored arena's agents take the slots they have
+ *   in the snapshot arena, and the arena's slot counters come from the snapshot too.  env_reset starts over at 0.
+ *   The slot space S(g) is the largest slot count of group g over all arenas in their current episode and over every
+ *   live snapshot's arenas.  It is therefore a bound that no device-side restore can exceed.  Only host-side calls change
+ *   it: env_reset, add_agents, snapshot_arenas and free_snapshot.  Read it with env_get_info(game, -1, "slot_space",
+ *   int[n_group]), which never waits, like "num_bound".
+ *   row_slot[r] = a * S + slot                int32 [num_bound(group)], may be NULL
+ *                 for each row r (the rows of env_set_action) below the device-side total of the group, a being the row's
+ *                 arena; -1 from the device-side total up to num_bound: the valid-row mask of a device consumer
+ *   slot_row[a][slot] = r                     int32 [num_arenas][S], may be NULL
+ *                 the row of the agent occupying the slot, or -1 when the slot is vacant (never placed in this episode,
+ *                 or its agent was culled).  A dead agent that has not been culled keeps its row.
+ * Either pointer may be NULL, but not both.  Both host pointers: the call waits for the counts.  Both CUDA device
+ * pointers: no synchronisation, no allocation, recordable into a CUDA graph, also after a restore from a device src
+ * inside the graph.  Returns -1, sets magent_b200_last_error and writes nothing for a bad group handle, two NULL
+ * pointers, pointers that mix host and CUDA device memory, or a backend without the kernel.  magent_b200_select_arena
+ * does not apply. */
+int magent_b200_get_slots(EnvHandle game, GroupHandle group, int *row_slot, int *slot_row);
 /* compact observation hand-off (SURVEY.md 8f rank 2): same call, layout and pointer rules as env_get_observation
  * (reference src/runtime_api.h:35), but every element is an IEEE binary16 = the float32 value rounded to
  * nearest-even.  buffer[0] = view [n][view_h][view_w][n_channel], buffer[1] = feature [n][feature_size];

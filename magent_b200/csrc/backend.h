@@ -93,6 +93,17 @@ __attribute__((weak)) void launch_mean_action(Ctx *, const EngineDev *dE, const 
 __attribute__((weak)) void launch_neighbours(Ctx *, const EngineDev *dE, const EngineDev &hE, const NbrCell *lut,
                                              unsigned curmask, int group, int of, int k, int *idx, int *rel, int *count,
                                              int n_total);
+// Stable slots of `group` (slot_phases.h): row_slot[r] = a * S + slot for every row r below the device-side total, -1
+// from there up to n_bound, and slot_row[a][slot] = the row of the agent in that slot, -1 where none is; either may be
+// null, both are device buffers.  `T` is the engine's SlotDev block, a device pointer.  n_bound is the host's bound of
+// the rows (num_bound): the device-side offsets decide.  launch_restore_slots copies, for every arena launch_restore
+// (same src and done rules) is about to restore, the first SLOT_HDR + snap_id_cap words of the snapshot table's row s
+// into the live row; it runs before launch_restore, which changes the done words.  Weak like launch_neighbours: the
+// engine refuses get_slots without them.
+__attribute__((weak)) void launch_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
+                                        unsigned curmask, int group, int S, int *row_slot, int *slot_row, int n_bound);
+__attribute__((weak)) void launch_restore_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
+                                                const int *snap_tab, int snap_id_cap, const int *src);
 // clear_dead: asynchronous read-back of the [G][A+1] offset table (launch_offsets) into page-locked memory
 void counts_fetch_begin(Ctx *, const int *dev_off, size_t n_ints);
 const int *counts_fetch_wait(Ctx *);     // blocks until the fetch has landed; valid until the next counts_fetch_begin

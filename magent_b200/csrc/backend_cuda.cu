@@ -29,6 +29,7 @@ namespace mg { __device__ long long mg_phase_clock[8 * 32]; }
 #include "obs_phases.h"
 #include "mask_phases.h"
 #include "nbr_phases.h"
+#include "slot_phases.h"
 
 namespace cg = cooperative_groups;
 
@@ -1963,6 +1964,67 @@ void launch_restore(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned c
     post_launch("restore_kernel");
     restore_finish_kernel<<<1, 1024, 0, c->stream>>>(dE, src, S.done);
     post_launch("restore_finish_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
+// stable slots (magent_b200_get_slots, slot_phases.h).  One CTA per arena: the arena's [S] block of slot_row is filled
+// with -1, then every row of the arena (the device-side offsets say how many) looks its agent's id up in the slot table,
+// writes a * S + slot to row_slot and scatters its row into slot_row.  Consecutive threads take consecutive rows and
+// slots, so the fill and the row_slot stores are coalesced, and so is the scatter while slots still follow the rows
+// (culls only open gaps).  The rows from the device-side total up to n_bound get -1, dealt over every CTA.
+constexpr int SLOT_THREADS = 256;
+
+__global__ void __launch_bounds__(SLOT_THREADS) slots_kernel(const int *off, const int *ids, int cap, const SlotDev *T,
+                                                             int A, int S, int *row_slot, int *slot_row, int n_bound) {
+    const int a = blockIdx.x;
+    const int *tab = T->tab;
+    const int id_cap = T->id_cap;
+    if (slot_row) {
+        for (int q = threadIdx.x; q < S; q += SLOT_THREADS) slot_row[(long)a * S + q] = -1;
+        __syncthreads();
+    }
+    const int o0 = off[a];
+    const int cnt = min(off[a + 1] - o0, n_bound - o0);         // never beyond the caller's buffer
+    const int *id = ids + (long)a * cap;
+    for (int i = threadIdx.x; i < cnt; i += SLOT_THREADS) {
+        const int flat = slot_flat(tab, id_cap, a, __ldg(id + i), S);
+        if (row_slot) row_slot[o0 + i] = flat;
+        if (slot_row && flat >= 0) slot_row[flat] = o0 + i;
+    }
+    if (row_slot)
+        for (int r = off[A] + a * SLOT_THREADS + threadIdx.x; r < n_bound; r += A * SLOT_THREADS) row_slot[r] = -1;
+}
+
+void launch_slots(Ctx *c, const EngineDev *, const EngineDev &hE, const SlotDev *T, unsigned curmask, int group, int S,
+                  int *row_slot, int *slot_row, int n_bound) {
+    DeviceGuard guard(c);
+    const GroupDev &D = hE.grp[group];
+    slots_kernel<<<(unsigned)hE.A, SLOT_THREADS, 0, c->stream>>>(hE.off + (size_t)group * (hE.A + 1),
+                                                                 D.soa[(curmask >> group) & 1u].id, D.cap, T, hE.A, S,
+                                                                 row_slot, slot_row, n_bound);
+    post_launch("slots_kernel");
+}
+
+// the slot rows of the arenas a restore is about to replace (restore_source decides, before restore_finish_kernel
+// rewrites the done words): the snapshot row's counters and id -> slot entries, at most the live table's width
+__global__ void __launch_bounds__(SLOT_THREADS) restore_slots_kernel(const SlotDev *T, const int *snap_tab,
+                                                                     int snap_id_cap, const int *src, const int *done,
+                                                                     int A) {
+    const int a = blockIdx.x;
+    const int s = restore_source(src, done, A, a);
+    if (s < 0) return;
+    const int id_cap = T->id_cap;
+    int *dst = T->tab + (long)a * slot_row_stride(id_cap);
+    const int *from = snap_tab + (long)s * slot_row_stride(snap_id_cap);
+    const long n = slot_row_stride(min(id_cap, snap_id_cap));
+    for (long q = threadIdx.x; q < n; q += SLOT_THREADS) dst[q] = __ldg(from + q);
+}
+
+void launch_restore_slots(Ctx *c, const EngineDev *, const EngineDev &hE, const SlotDev *T, const int *snap_tab,
+                          int snap_id_cap, const int *src) {
+    DeviceGuard guard(c);
+    restore_slots_kernel<<<(unsigned)hE.A, SLOT_THREADS, 0, c->stream>>>(T, snap_tab, snap_id_cap, src, hE.done, hE.A);
+    post_launch("restore_slots_kernel");
 }
 
 __global__ void __launch_bounds__(256) arena_done_kernel(const EngineDev *gE, int *out) {

@@ -240,6 +240,18 @@ struct alignas(16) NbrCell {
     int off, delta, key, cell;
 };
 
+// Stable agent slots (magent_b200_get_slots, slot_phases.h).  The table has one row of SLOT_HDR + id_cap ints per arena:
+// words [0, MG_MAX_GROUPS) are the arena's slot counters (agents of each group placed since its last reset), word
+// SLOT_HDR + id the slot of the agent with that id.  Ids are unique per arena and restart at 0 with env_reset, so a
+// restore copies a row prefix and nothing else changes it between host-side placements.  It lives outside EngineDev and
+// outside ArenaHdr, so no step, cull or render kernel sees it; this block is allocated once per engine and names the
+// current table, which grows with the largest id counter while a captured graph keeps pointing at the block.
+enum { SLOT_HDR = MG_MAX_GROUPS };
+struct SlotDev {
+    int *tab;                                 // [A][SLOT_HDR + id_cap]
+    int id_cap;
+};
+
 enum InfoKind { INFO_ID = 0, INFO_POS, INFO_ALIVE, INFO_REWARD, INFO_ACTION_SCATTER, INFO_HP };
 
 }  // namespace mg

@@ -2,6 +2,7 @@
 #include "engine.h"
 #include "step_phases.h"
 #include "nbr_phases.h"
+#include "slot_phases.h"
 
 #include <math.h>
 #include <stdarg.h>
@@ -127,6 +128,8 @@ Engine::~Engine() {
     for (ArenaSnapshot &sn : snaps_)
         for (void *p : sn.allocs) be::dfree(bx_, p);
     free_device();
+    if (d_slot_tab_) be::dfree(bx_, d_slot_tab_);
+    if (d_slot_dev_) be::dfree(bx_, d_slot_dev_);
     if (h_feat_stage_) be::host_free(h_feat_stage_);
     if (bx_) be::destroy(bx_);
 }
@@ -458,6 +461,8 @@ void Engine::reset() {                                // GridWorld.cc:72-118, Ma
     nsep_ = large_map_ ? ((long)W_ * H_ > 1000 * 1000 ? 16 : 8) : 1;
     for (auto &ar : arenas_) {
         ar.id_counter = 0;
+        ar.slot_of_id.clear();
+        for (int &c : ar.slot_ct) c = 0;
         ar.done = 0;
         ar.occ.assign((size_t)W_ * H_, OCC_EMPTY);
         ar.food.assign(food_mode_ ? (size_t)W_ * H_ : 0, 0.0f);
@@ -470,6 +475,7 @@ void Engine::reset() {                                // GridWorld.cc:72-118, Ma
     was_reset_ = true;
     order_.clear();
     refresh_host_counts();
+    update_slot_space();
 }
 
 bool Engine::host_is_blank(const HostArena &ar, int x, int y, int w, int h) const {   // Map.cc:454-470
@@ -510,6 +516,7 @@ int Engine::host_add_agent(HostArena &ar, int g, int x, int y, int dir) {       
     if (i >= (1 << 23)) fatal("too many agents in one group of one arena (max %d)", 1 << 23);
     hg.resize(i + 1);
     hg.x[i] = x; hg.y[i] = y; hg.id[i] = ar.id_counter++;
+    ar.slot_of_id.push_back(ar.slot_ct[g]++);           // the id's slot (slot_phases.h); ids are handed out in order
     hg.act[i] = t.n_action;                           // "dangerous here !" (GridWorld.h:140)
     hg.op_obj[i] = -1;
     hg.hp[i] = t.hp;
@@ -571,6 +578,7 @@ void Engine::add_agents(int group, int n, const char *method,
         }
     }
     refresh_host_counts();
+    update_slot_space();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -684,6 +692,53 @@ void Engine::upload_nbr_luts(bool force) {
     if (!force && same) return;
     if (!lut.empty()) be::h2d(bx_, d_nbr_lut_, lut.data(), lut.size() * sizeof(NbrCell));
     nbr_lut_.swap(lut);
+}
+
+// The slot table of the host image.  Its width covers every id an arena or a live snapshot's arena has handed out, so a
+// restore never needs more; it only grows (by half at least, so that mid-episode placements rarely re-allocate), and the
+// SlotDev block that names it keeps its address.
+void Engine::upload_slots() {
+    int need = 0;
+    for (const HostArena &ar : arenas_) need = std::max(need, ar.id_counter);
+    for (const ArenaSnapshot &sn : snaps_)
+        if (sn.live) need = std::max(need, sn.max_ids);
+    if (!d_slot_dev_) d_slot_dev_ = (SlotDev *)be::dmalloc(bx_, sizeof(SlotDev));
+    if (!d_slot_tab_ || need > slot_id_cap_) {
+        if (d_slot_tab_) be::dfree(bx_, d_slot_tab_);
+        const int want = std::max(need, slot_id_cap_ + slot_id_cap_ / 2);
+        slot_id_cap_ = std::max(64, (want + 63) / 64 * 64);
+        d_slot_tab_ = (int *)be::dmalloc(bx_, (size_t)A_ * slot_row_stride(slot_id_cap_) * 4);
+        const SlotDev T = {d_slot_tab_, slot_id_cap_};
+        be::h2d(bx_, d_slot_dev_, &T, sizeof T);
+    }
+    const long ld = slot_row_stride(slot_id_cap_);
+    std::vector<int> tab((size_t)A_ * ld, -1);
+    for (int a = 0; a < A_; ++a) {
+        int *row = tab.data() + a * ld;
+        std::copy(arenas_[a].slot_ct, arenas_[a].slot_ct + SLOT_HDR, row);
+        std::copy(arenas_[a].slot_of_id.begin(), arenas_[a].slot_of_id.end(), row + SLOT_HDR);
+    }
+    be::h2d(bx_, d_slot_tab_, tab.data(), tab.size() * 4);
+}
+
+// S(g): the largest slot count of group g over the arenas as they are now and over the arenas of every snapshot a restore
+// may copy in.  Device restores cannot exceed it, so only the host-side calls that can change it recompute it.
+void Engine::update_slot_space() {
+    const int Gn = G();
+    slot_space_.assign(Gn, 0);
+    std::vector<int> tab;
+    const long ld = slot_row_stride(slot_id_cap_);
+    if (where_ == DEVICE) {
+        tab.resize((size_t)A_ * ld);
+        be::d2h(bx_, tab.data(), d_slot_tab_, tab.size() * 4);
+    }
+    for (int a = 0; a < A_; ++a)
+        for (int g = 0; g < Gn; ++g)
+            slot_space_[g] = std::max(slot_space_[g], where_ == DEVICE ? tab[a * ld + g] : arenas_[a].slot_ct[g]);
+    const int pad = view_pad();
+    for (const ArenaSnapshot &sn : snaps_)
+        if (sn.live && snap_matches(sn, pad))
+            for (int g = 0; g < Gn; ++g) slot_space_[g] = std::max(slot_space_[g], sn.slot_max[g]);
 }
 
 void Engine::to_device() {
@@ -912,6 +967,7 @@ void Engine::to_device() {
         be::h2d(bx_, hE_.done, done.data(), done.size() * 4);
         be::h2d(bx_, hE_.off, h_off_.data(), h_off_.size() * 4);
     }
+    upload_slots();
     be::h2d(bx_, dE_, &hE_, sizeof(EngineDev));
     ++state_version_;
     may_have_dead_ = true;                            // conservative: the first clear_dead after an upload re-reads the counts
@@ -963,6 +1019,16 @@ void Engine::to_host(bool keep_device_authoritative) {
         arenas_[a].rng = hdr[a].rng;
         arenas_[a].done = hdr[a].done;
         arenas_[a].id_counter = hdr[a].id_counter;
+    }
+    {   // the slot table: restores may have replaced rows
+        const long ld = slot_row_stride(slot_id_cap_);
+        std::vector<int> tab((size_t)A_ * ld);
+        be::d2h(bx_, tab.data(), d_slot_tab_, tab.size() * 4);
+        for (int a = 0; a < A_; ++a) {
+            const int *row = tab.data() + a * ld;
+            std::copy(row, row + SLOT_HDR, arenas_[a].slot_ct);
+            arenas_[a].slot_of_id.assign(row + SLOT_HDR, row + SLOT_HDR + arenas_[a].id_counter);
+        }
     }
     if (!keep_device_authoritative) where_ = HOST;
 }
@@ -1104,6 +1170,13 @@ void Engine::set_counts(const std::vector<int> &c) {
             h_off_[(size_t)g * (A_ + 1) + a + 1] = h_off_[(size_t)g * (A_ + 1) + a] + c[(size_t)g * A_ + a];
 }
 
+int Engine::num_bound(int g) const {
+    const std::vector<int> floor = restore_floor();
+    long long n = 0;
+    for (int a = 0; a < A_; ++a) n += std::max(count(g, a), floor[g]);
+    return (int)n;
+}
+
 void Engine::raise_counts(const std::vector<int> &floor) {
     std::vector<int> c((size_t)G() * A_);
     for (int g = 0; g < G(); ++g)
@@ -1160,7 +1233,22 @@ int Engine::snapshot_arenas() {
         snap_copy(bx_, sn.allocs, S.last_op, L.last_op, n); snap_copy(bx_, sn.allocs, S.flags, L.flags, n);
         snap_copy(bx_, sn.allocs, S.dir, L.dir, n);
     }
+    {   // the slot table, and the id and slot counts a restore from it can bring in
+        const long ld = slot_row_stride(slot_id_cap_);
+        snap_copy(bx_, sn.allocs, sn.slot_tab, (const int *)d_slot_tab_, (size_t)A_ * ld);
+        sn.slot_id_cap = slot_id_cap_;
+        std::vector<int> tab((size_t)A_ * ld);
+        be::d2h(bx_, tab.data(), d_slot_tab_, tab.size() * 4);
+        std::vector<ArenaHdr> hdr(A_);
+        be::d2h(bx_, hdr.data(), hE_.hdr, sizeof(ArenaHdr) * A_);
+        sn.slot_max.assign(Gn, 0);
+        for (int a = 0; a < A_; ++a) {
+            sn.max_ids = std::max(sn.max_ids, hdr[a].id_counter);
+            for (int g = 0; g < Gn; ++g) sn.slot_max[g] = std::max(sn.slot_max[g], tab[a * ld + g]);
+        }
+    }
     snaps_.push_back(sn);                             // ids are never reused: a freed id stays unknown
+    update_slot_space();
     return (int)snaps_.size() - 1;
 }
 
@@ -1171,6 +1259,7 @@ int Engine::free_snapshot(int id) {
     if (be::capturing(bx_)) return refuse("free_snapshot is not possible while a CUDA graph is being captured");
     for (void *p : sn.allocs) be::dfree(bx_, p);
     sn = ArenaSnapshot();
+    update_slot_space();
     return 0;
 }
 
@@ -1202,6 +1291,8 @@ int Engine::restore_arenas(int id, const int *src, int keep_rng) {
         io_[IO_H2D] += (long long)A_ * 4;
         d_src = st;
     }
+    // the slot rows first: launch_restore rewrites the done words a null src decides by
+    if (be::launch_restore_slots) be::launch_restore_slots(bx_, dE_, hE_, d_slot_dev_, sn.slot_tab, sn.slot_id_cap, d_src);
     be::launch_restore(bx_, dE_, hE_, curmask_, sn.dev, d_src, keep_rng ? 1 : 0);
     ++state_version_;
     may_have_dead_ = true;
@@ -1344,6 +1435,31 @@ int Engine::get_neighbours(int group, int of, int k, int *idx, int *rel, int *co
     if (rel) be::d2h(bx_, rel, st + idx_bytes, rel_bytes);
     if (count) be::d2h(bx_, count, st + idx_bytes + rel_bytes, count_bytes);
     io_[IO_D2H] += (long long)(idx_bytes + rel_bytes + count_bytes);
+    return 0;
+}
+
+// The stable slots of one group.  Same pointer discipline as get_mean_action: device buffers take one kernel sized by the
+// host's bound and clamped by the device-side counts, host buffers settle the counts and go through the i/o staging
+// (row_slot, num_bound ints, and slot_row, A * S ints, share one staging block).
+int Engine::get_slots(int group, int *row_slot, int *slot_row) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_slots", group);
+    if (!row_slot && !slot_row) return refuse("get_slots needs a row_slot or a slot_row buffer");
+    if (!be::launch_slots || !be::launch_restore_slots) return refuse("the %s backend has no slots kernel", be::name());
+    const bool dev = be::is_device_ptr(row_slot ? row_slot : slot_row);
+    if (row_slot && slot_row && be::is_device_ptr(slot_row) != dev)
+        return refuse("get_slots: row_slot and slot_row must both be host memory or both CUDA device memory");
+    to_device();
+    if (!dev) settle_counts();
+    const int S = group < (int)slot_space_.size() ? slot_space_[group] : 0, nb = num_bound(group);
+    const size_t rows_n = row_slot ? (size_t)nb : 0, map_n = slot_row ? (size_t)A_ * S : 0;
+    if (rows_n + map_n == 0) return 0;
+    if (dev) { be::launch_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, row_slot, slot_row, nb); return 0; }
+    int *st = (int *)io_stage((rows_n + map_n) * 4);
+    be::launch_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, row_slot ? st : nullptr,
+                     slot_row ? st + rows_n : nullptr, nb);
+    if (row_slot) be::d2h(bx_, row_slot, st, rows_n * 4);
+    if (slot_row) be::d2h(bx_, slot_row, st + rows_n, map_n * 4);
+    io_[IO_D2H] += (long long)(rows_n + map_n) * 4;
     return 0;
 }
 
@@ -1613,12 +1729,11 @@ int Engine::get_info(int group, const char *name, void *void_buffer) {         /
         return 0;
     }
     if (strequ(name, "num_bound")) {                    // extension: per group, records a device-pointer call may write
-        const std::vector<int> floor = restore_floor(); // before the counts next settle (no waiting here)
-        for (int g = 0; g < G(); ++g) {
-            long long n = 0;
-            for (int a = 0; a < A_; ++a) n += std::max(count(g, a), floor[g]);
-            ib[g] = (int)n;
-        }
+        for (int g = 0; g < G(); ++g) ib[g] = num_bound(g);     // before the counts next settle (no waiting here)
+        return 0;
+    }
+    if (strequ(name, "slot_space")) {                   // extension: per group, S of magent_b200_get_slots (no waiting)
+        for (int g = 0; g < G(); ++g) ib[g] = g < (int)slot_space_.size() ? slot_space_[g] : 0;
         return 0;
     }
     if (strequ(name, "arena_rng")) {                    // extension: uint32 minstd state of every arena

@@ -61,6 +61,10 @@ struct HostArena {
     uint32_t rng = 1;
     int id_counter = 0;
     int done = 0;
+    // stable slots (slot_phases.h): slot_of_id[id] for every id handed out since the last reset (size id_counter), and
+    // per group the slots handed out
+    std::vector<int> slot_of_id;
+    int slot_ct[MG_MAX_GROUPS] = {0};
 };
 
 // a copy of every arena's state in HBM (Engine::snapshot_arenas): its own allocations, outside dev_allocs_, so that
@@ -75,6 +79,11 @@ struct ArenaSnapshot {
     std::vector<int> n;                 // [G][A] agents per group and arena
     std::vector<int> max_n;             // [G] largest per-arena count
     SnapDev dev;
+    // the slot table at the time ([A][SLOT_HDR + slot_id_cap], in allocs) and what a restore from it can bring in: the
+    // largest id counter and per group the largest slot count of its arenas
+    int *slot_tab = nullptr;
+    int slot_id_cap = 0, max_ids = 0;
+    std::vector<int> slot_max;
     std::vector<void *> allocs;
 };
 
@@ -129,6 +138,9 @@ public:
     // the first k neighbours of group `of`, nearest first (nbr_phases.h nbr_cell_key): int [n][k] rows of `of`, int
     // [n][k][2] view cells and int [n] neighbour counts (rel and count may be null).  -1 and the last error when refused.
     int get_neighbours(int group, int of, int k, int *idx, int *rel, int *count);
+    // stable slots (slot_phases.h): int [num_bound] row -> a * S + slot and int [A][S] slot -> row of one group, S =
+    // slot_space(group); either may be null, not both.  -1 and the last error when refused.
+    int get_slots(int group, int *row_slot, int *slot_row);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads
@@ -192,6 +204,16 @@ private:
     std::vector<size_t> nbr_lut_base_;
     std::vector<unsigned char> nbr_key_fits_;
     void upload_nbr_luts(bool force);
+    // stable slots: the live table ([A][SLOT_HDR + slot_id_cap_], grow-only, outside dev_allocs_ so that a re-allocation
+    // of the device image does not drop it), the SlotDev block naming it (allocated once, so captured graphs stay valid
+    // when the table grows), and slot_space_[g] = S(g) as the last reset, add_agents, snapshot_arenas or free_snapshot
+    // left it
+    int *d_slot_tab_ = nullptr;
+    int slot_id_cap_ = 0;
+    SlotDev *d_slot_dev_ = nullptr;
+    std::vector<int> slot_space_;
+    void upload_slots();
+    void update_slot_space();
     size_t view_stage_bytes_ = 0, feat_stage_bytes_ = 0;
     void *d_io_stage_ = nullptr; size_t io_stage_bytes_ = 0;
     void *h_feat_stage_ = nullptr; size_t h_feat_stage_bytes_ = 0;      // page-locked staging of the feature rows (host path)
@@ -226,6 +248,7 @@ private:
     std::vector<int> restore_floor() const;          // [G] largest count any usable snapshot can restore an arena to
     void set_counts(const std::vector<int> &c);           // h_off_ from per-arena counts c[G][A]
     void raise_counts(const std::vector<int> &floor);     // h_off_ counts to at least floor[g] in every arena
+    int num_bound(int g) const;         // the "num_bound" info key: rows a device-pointer call may write before the counts settle
     bool capture_floor_ = false;        // the capture in progress sizes its launches for restores (graph_begin)
 
     void ensure_backend();

@@ -114,6 +114,9 @@ MG_API int magent_b200_get_neighbours(EnvHandle game, GroupHandle group, GroupHa
                                       int *count) {
     return E(game)->get_neighbours(group, of, k, idx, rel, count);
 }
+MG_API int magent_b200_get_slots(EnvHandle game, GroupHandle group, int *row_slot, int *slot_row) {
+    return E(game)->get_slots(group, row_slot, slot_row);
+}
 MG_API int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **buffer) {
     E(game)->get_observation(group, buffer, 1);
     return 0;

@@ -717,6 +717,70 @@ class GridWorld(Environment):
                     "get_neighbours")
         return idx[:n], None if rel is None else rel[:n], None if count is None else count[:n]
 
+    def get_slot_space(self, handle):
+        """S, the slot space of the group: slots run over [0, S) in every arena (include/magent_b200_ext.h
+        magent_b200_get_slots has the definition).  Only reset, add_agents, snapshot_arenas and free_snapshot change it;
+        nothing waits for the device."""
+        buf = np.empty((len(self.group_handles),), dtype=np.int32)
+        self._lib.env_get_info(self.game, -1, b"slot_space", buf.ctypes.data)
+        return int(buf[self._hv(handle)])
+
+    def get_slots(self, handle):
+        """(row_slot int32 (n,), slot_row int32 (num_arenas, S)): the stable slot of every agent of the group.  An agent's
+        slot is the number of agents of its group placed into its arena before it since the last reset; it survives
+        clear_dead, and a restored arena's agents keep the slots they have in the snapshot.  row_slot[r] = a * S + slot
+        for row r (the order of set_action), a its arena; slot_row[a, slot] = the row of the agent in that slot, -1 when
+        the slot is vacant.  Both arrays are cached receive buffers: valid until the next call."""
+        g = self._hv(handle)
+        n = self.get_num(handle)                 # settles the counts, so the bound below is the call's
+        bound = self.get_num_bound(handle)
+        S = self.get_slot_space(handle)
+        block = self._blocks.get((g, "slots"))
+        if block is None:
+            block = self._blocks[(g, "slots")] = _HostBlock(self._lib)
+        raw = block.view((bound + self.num_arenas * S,), np.int32)
+        row_slot, slot_row = raw[:bound], raw[bound:].reshape(self.num_arenas, S)
+        self._check(self._lib.magent_b200_get_slots(self.game, g, row_slot.ctypes.data, slot_row.ctypes.data),
+                    "get_slots")
+        return row_slot[:n], slot_row
+
+    def get_slots_torch(self, handle, out=None):
+        """the stable slots (see get_slots) written straight into CUDA tensors, without waiting for the device: returns
+        (row_slot int32 (num_bound,), slot_row int32 (num_arenas, S)).  Entries of row_slot from the device-side count of
+        the group on are -1, so it is also the valid-row mask of the group's row-ordered outputs.  Scatter rows into
+        slots with x[slot_row.clamp(min=0)] and gather slot-ordered actions back with act_s.view(-1)[row_slot.clamp(min=0)]
+        (INTEGRATION.md §4).
+
+        out: a caller-owned pair (row_slot, slot_row) of contiguous CUDA int32 tensors, of shapes (rows,) with at least
+        get_num_bound(handle) rows and (num_arenas, get_slot_space(handle)); needed to record the call into a CUDA graph
+        (capture_graph), since the call then allocates nothing.  Either may be None: it is then not written, and None comes
+        back in its place.  The first get_num_bound(handle) entries of row_slot are written."""
+        import torch
+        g = self._hv(handle)
+        bound = self.get_num_bound(handle)
+        S = self.get_slot_space(handle)
+        if out is None:
+            row_slot = torch.empty((bound,), dtype=torch.int32, device="cuda")
+            slot_row = torch.empty((self.num_arenas, S), dtype=torch.int32, device="cuda")
+        else:
+            if not isinstance(out, (tuple, list)) or len(out) != 2 or (out[0] is None and out[1] is None):
+                raise ValueError("out must be a (row_slot, slot_row) pair of CUDA tensors, at most one of them None")
+            row_slot, slot_row = out
+            for t in (row_slot, slot_row):
+                if t is not None and (not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.int32 or
+                                      not t.is_contiguous()):
+                    raise ValueError("out must hold contiguous CUDA int32 tensors")
+            if row_slot is not None and (row_slot.dim() != 1 or row_slot.shape[0] < bound):
+                raise ValueError("row_slot must be of shape (rows,) with at least %d rows" % bound)
+            if slot_row is not None and tuple(slot_row.shape) != (self.num_arenas, S):
+                raise ValueError("slot_row must be of shape (%d, %d)" % (self.num_arenas, S))
+        # an empty tensor's pointer is NULL: it has nothing to receive
+        ptr = (lambda t: None if t is None or t.numel() == 0 else ctypes.c_void_p(t.data_ptr()))
+        if ptr(row_slot) is None and ptr(slot_row) is None:
+            return row_slot, slot_row
+        self._check(self._lib.magent_b200_get_slots(self.game, g, ptr(row_slot), ptr(slot_row)), "get_slots")
+        return row_slot, slot_row
+
     def get_counters(self):
         """int64 event counters accumulated on the device since construction"""
         buf = (ctypes.c_longlong * 16)()
