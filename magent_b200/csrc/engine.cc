@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <chrono>
 #include <fstream>
+#include <initializer_list>
 #include <set>
 #include <sstream>
 
@@ -621,6 +622,36 @@ void *Engine::io_stage(size_t bytes) {
         d_io_stage_ = be::dmalloc(bx_, io_stage_bytes_);
     }
     return d_io_stage_;
+}
+
+// The per-agent read-backs (get_reward, get_info's id/pos/alive/hp, get_action_mask, get_mean_action, get_neighbours,
+// get_slots) write into caller buffers that are all host memory or all CUDA device memory, the null ones aside.
+// out_memory says which: 1 device, 0 host, -1 refused.
+static int out_memory(const char *what, std::initializer_list<const void *> bufs) {
+    int dev = 0, host = 0;
+    for (const void *p : bufs) if (p) ++(be::is_device_ptr(p) ? dev : host);
+    const char *q = bufs.size() == 2 ? "both" : "all";
+    if (dev && host) return refuse("%s must %s be host memory or %s CUDA device memory", what, q, q);
+    return dev ? 1 : 0;
+}
+
+// launch(void **to) writes each wanted part to to[i] (nullptr: not wanted).  Device buffers: to[] are the caller's, the
+// launch is sized by the host's upper-bound counts and clamped by the device's, and nothing is staged, allocated or
+// waited for, so the call can be recorded into a CUDA graph.  Host buffers (the caller settled the counts): the wanted
+// parts are packed back to back in one i/o staging block, then each is copied back and counted in IO_D2H.  Nothing runs
+// when the wanted parts total 0 bytes.
+template <size_t N, class F> void Engine::read_back(bool dev, const OutPart (&parts)[N], F &&launch) {
+    void *to[N];
+    size_t bytes = 0;
+    for (size_t i = 0; i < N; ++i) { to[i] = parts[i].buf; bytes += parts[i].buf ? parts[i].bytes : 0; }
+    if (bytes == 0) return;
+    if (dev) { launch(to); return; }
+    char *st = (char *)io_stage(bytes);
+    for (size_t i = 0, off = 0; i < N; ++i)
+        if (parts[i].buf) { to[i] = st + off; off += parts[i].bytes; }
+    launch(to);
+    for (size_t i = 0; i < N; ++i)
+        if (parts[i].buf) { be::d2h(bx_, parts[i].buf, to[i], parts[i].bytes); io_[IO_D2H] += (long long)parts[i].bytes; }
 }
 
 // the padded observation planes cover the widest view window of any group, in any heading when agents can turn
@@ -1350,9 +1381,7 @@ void Engine::random_actions(int group, unsigned long long seed) {
     be::launch_random_actions(bx_, dE_, hE_, curmask_, group, seed * 0x9E3779B97F4A7C15ull + (++rand_calls_), n);
 }
 
-// Legal-action mask of one group.  A device buffer takes one kernel sized by the host's (upper-bound) counts and clamped
-// by the device's: no synchronisation, no allocation, recordable into a graph.  A host buffer needs the exact counts and
-// goes through the i/o staging like the other per-agent read-backs.
+// Legal-action mask of one group
 int Engine::get_action_mask(int group, unsigned char *buf) {
     if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_action_mask", group);
     if (!be::launch_action_mask) return refuse("the %s backend has no action-mask kernel", be::name());
@@ -1360,13 +1389,9 @@ int Engine::get_action_mask(int group, unsigned char *buf) {
     const bool dev = be::is_device_ptr(buf);
     if (!dev) settle_counts();
     const int n = total(group);
-    if (n == 0) return 0;
-    if (dev) { be::launch_action_mask(bx_, dE_, hE_, curmask_, group, buf, n); return 0; }
-    const size_t bytes = (size_t)n * group_type_[group]->n_action;
-    unsigned char *st = (unsigned char *)io_stage(bytes);
-    be::launch_action_mask(bx_, dE_, hE_, curmask_, group, st, n);
-    be::d2h(bx_, buf, st, bytes);
-    io_[IO_D2H] += (long long)bytes;
+    read_back(dev, {{buf, (size_t)n * group_type_[group]->n_action}}, [&](void **to) {
+        be::launch_action_mask(bx_, dE_, hE_, curmask_, group, (unsigned char *)to[0], n);
+    });
     return 0;
 }
 
@@ -1382,84 +1407,60 @@ int Engine::random_legal_actions(int group, unsigned long long seed) {
     return 0;
 }
 
-// Mean neighbour action of one group over the agents of group `of` it sees.  Same pointer discipline as
-// get_action_mask: device buffers take one kernel clamped by the device-side counts, host buffers settle the counts and go
-// through the i/o staging (mean and count share one staging block).
+// Mean neighbour action of one group over the agents of group `of` it sees
 int Engine::get_mean_action(int group, int of, float *mean, int *count) {
     if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_mean_action", group);
     if (of < 0 || of >= G()) return refuse("invalid group handle %d for `of` in get_mean_action", of);
     if (!be::launch_mean_action) return refuse("the %s backend has no mean-action kernel", be::name());
-    const bool dev = mean && be::is_device_ptr(mean);
-    if (mean && count && be::is_device_ptr(count) != dev)
-        return refuse("get_mean_action: mean and count must both be host memory or both CUDA device memory");
+    const int mem = out_memory("get_mean_action: mean and count", {mean, count});
+    if (mem < 0) return -1;
+    const bool dev = mean && mem;       // a null mean counts as host memory (refused below unless the group is empty)
     to_device();
     if (!dev) settle_counts();
     const int n = total(group);
     if (n == 0) return 0;
     if (!mean) return refuse("get_mean_action needs a mean buffer");
-    if (dev) { be::launch_mean_action(bx_, dE_, hE_, curmask_, group, of, mean, count, n); return 0; }
-    const size_t mean_bytes = (size_t)n * group_type_[of]->n_action * 4, count_bytes = count ? (size_t)n * 4 : 0;
-    char *st = (char *)io_stage(mean_bytes + count_bytes);
-    be::launch_mean_action(bx_, dE_, hE_, curmask_, group, of, (float *)st, count ? (int *)(st + mean_bytes) : nullptr, n);
-    be::d2h(bx_, mean, st, mean_bytes);
-    if (count) be::d2h(bx_, count, st + mean_bytes, count_bytes);
-    io_[IO_D2H] += (long long)(mean_bytes + count_bytes);
+    read_back(dev, {{mean, (size_t)n * group_type_[of]->n_action * 4}, {count, (size_t)n * 4}}, [&](void **to) {
+        be::launch_mean_action(bx_, dE_, hE_, curmask_, group, of, (float *)to[0], (int *)to[1], n);
+    });
     return 0;
 }
 
-// The first k neighbours of one group in group `of`, nearest first.  Same pointer discipline as get_mean_action: device
-// buffers take one kernel clamped by the device-side counts, host buffers settle the counts and go through the i/o
-// staging (idx, rel and count share one staging block).
+// The first k neighbours of one group in group `of`, nearest first
 int Engine::get_neighbours(int group, int of, int k, int *idx, int *rel, int *count) {
     if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_neighbours", group);
     if (of < 0 || of >= G()) return refuse("invalid group handle %d for `of` in get_neighbours", of);
     if (k < 1 || k > 32) return refuse("get_neighbours: k = %d is outside [1, 32]", k);
     if (!idx) return refuse("get_neighbours needs an idx buffer");
     if (!be::launch_neighbours) return refuse("the %s backend has no neighbours kernel", be::name());
-    const bool dev = be::is_device_ptr(idx);
-    if ((rel && be::is_device_ptr(rel) != dev) || (count && be::is_device_ptr(count) != dev))
-        return refuse("get_neighbours: idx, rel and count must all be host memory or all CUDA device memory");
+    const int mem = out_memory("get_neighbours: idx, rel and count", {idx, rel, count});
+    if (mem < 0) return -1;
     to_device();
     if (!nbr_key_fits_[group])
         return refuse("get_neighbours: the view of group %d is too large to order its cells by an int key", group);
-    if (!dev) settle_counts();
+    if (!mem) settle_counts();
     const int n = total(group);
-    if (n == 0) return 0;
-    const NbrCell *lut = d_nbr_lut_ + nbr_lut_base_[group];
-    if (dev) { be::launch_neighbours(bx_, dE_, hE_, lut, curmask_, group, of, k, idx, rel, count, n); return 0; }
-    const size_t idx_bytes = (size_t)n * k * 4, rel_bytes = rel ? 2 * idx_bytes : 0, count_bytes = count ? (size_t)n * 4 : 0;
-    char *st = (char *)io_stage(idx_bytes + rel_bytes + count_bytes);
-    be::launch_neighbours(bx_, dE_, hE_, lut, curmask_, group, of, k, (int *)st, rel ? (int *)(st + idx_bytes) : nullptr,
-                          count ? (int *)(st + idx_bytes + rel_bytes) : nullptr, n);
-    be::d2h(bx_, idx, st, idx_bytes);
-    if (rel) be::d2h(bx_, rel, st + idx_bytes, rel_bytes);
-    if (count) be::d2h(bx_, count, st + idx_bytes + rel_bytes, count_bytes);
-    io_[IO_D2H] += (long long)(idx_bytes + rel_bytes + count_bytes);
+    const size_t idx_bytes = (size_t)n * k * 4;
+    read_back(mem == 1, {{idx, idx_bytes}, {rel, 2 * idx_bytes}, {count, (size_t)n * 4}}, [&](void **to) {
+        be::launch_neighbours(bx_, dE_, hE_, d_nbr_lut_ + nbr_lut_base_[group], curmask_, group, of, k, (int *)to[0],
+                              (int *)to[1], (int *)to[2], n);
+    });
     return 0;
 }
 
-// The stable slots of one group.  Same pointer discipline as get_mean_action: device buffers take one kernel sized by the
-// host's bound and clamped by the device-side counts, host buffers settle the counts and go through the i/o staging
-// (row_slot, num_bound ints, and slot_row, A * S ints, share one staging block).
+// The stable slots of one group
 int Engine::get_slots(int group, int *row_slot, int *slot_row) {
     if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_slots", group);
     if (!row_slot && !slot_row) return refuse("get_slots needs a row_slot or a slot_row buffer");
     if (!be::launch_slots || !be::launch_restore_slots) return refuse("the %s backend has no slots kernel", be::name());
-    const bool dev = be::is_device_ptr(row_slot ? row_slot : slot_row);
-    if (row_slot && slot_row && be::is_device_ptr(slot_row) != dev)
-        return refuse("get_slots: row_slot and slot_row must both be host memory or both CUDA device memory");
+    const int mem = out_memory("get_slots: row_slot and slot_row", {row_slot, slot_row});
+    if (mem < 0) return -1;
     to_device();
-    if (!dev) settle_counts();
+    if (!mem) settle_counts();
     const int S = group < (int)slot_space_.size() ? slot_space_[group] : 0, nb = num_bound(group);
-    const size_t rows_n = row_slot ? (size_t)nb : 0, map_n = slot_row ? (size_t)A_ * S : 0;
-    if (rows_n + map_n == 0) return 0;
-    if (dev) { be::launch_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, row_slot, slot_row, nb); return 0; }
-    int *st = (int *)io_stage((rows_n + map_n) * 4);
-    be::launch_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, row_slot ? st : nullptr,
-                     slot_row ? st + rows_n : nullptr, nb);
-    if (row_slot) be::d2h(bx_, row_slot, st, rows_n * 4);
-    if (slot_row) be::d2h(bx_, slot_row, st + rows_n, map_n * 4);
-    io_[IO_D2H] += (long long)(rows_n + map_n) * 4;
+    read_back(mem == 1, {{row_slot, (size_t)nb * 4}, {slot_row, (size_t)A_ * S * 4}}, [&](void **to) {
+        be::launch_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, (int *)to[0], (int *)to[1], nb);
+    });
     return 0;
 }
 
@@ -1496,14 +1497,12 @@ void Engine::step(int *done) {                                        // GridWor
 void Engine::get_reward(int group, float *buf) {                      // GridWorld.cc:694-704
     check_group(group, "GridWorld::get_reward");
     to_device();
-    if (!be::is_device_ptr(buf)) settle_counts();
+    const bool dev = be::is_device_ptr(buf);
+    if (!dev) settle_counts();
     const int n = total(group);
-    if (n == 0) return;
-    if (be::is_device_ptr(buf)) { be::launch_info(bx_, dE_, hE_, curmask_, INFO_REWARD, group, buf, n); return; }
-    void *st = io_stage((size_t)n * 4);
-    be::launch_info(bx_, dE_, hE_, curmask_, INFO_REWARD, group, st, n);
-    be::d2h(bx_, buf, st, (size_t)n * 4);
-    io_[IO_D2H] += (long long)n * 4;
+    read_back(dev, {{buf, (size_t)n * 4}}, [&](void **to) {
+        be::launch_info(bx_, dE_, hE_, curmask_, INFO_REWARD, group, to[0], n);
+    });
 }
 
 void Engine::clear_dead() {                                           // GridWorld.cc:633-665
@@ -1755,13 +1754,11 @@ int Engine::get_info(int group, const char *name, void *void_buffer) {         /
         check_group(group, "get_info");
         to_device();
         const int n = total(group);
-        if (n == 0) return 0;
-        int kind = strequ(name, "id") ? INFO_ID : strequ(name, "pos") ? INFO_POS : strequ(name, "alive") ? INFO_ALIVE : INFO_HP;
-        size_t bytes = kind == INFO_POS ? (size_t)n * 8 : kind == INFO_ALIVE ? (size_t)n : (size_t)n * 4;
-        if (be::is_device_ptr(void_buffer)) { be::launch_info(bx_, dE_, hE_, curmask_, kind, group, void_buffer, n); return 0; }
-        void *st = io_stage(bytes);
-        be::launch_info(bx_, dE_, hE_, curmask_, kind, group, st, n);
-        be::d2h(bx_, void_buffer, st, bytes);
+        const int kind = strequ(name, "id") ? INFO_ID : strequ(name, "pos") ? INFO_POS : strequ(name, "alive") ? INFO_ALIVE : INFO_HP;
+        const size_t bytes = kind == INFO_POS ? (size_t)n * 8 : kind == INFO_ALIVE ? (size_t)n : (size_t)n * 4;
+        read_back(be::is_device_ptr(void_buffer), {{void_buffer, bytes}}, [&](void **to) {
+            be::launch_info(bx_, dE_, hE_, curmask_, kind, group, to[0], n);
+        });
     } else if (strequ(name, "arena_num")) {
         check_group(group, "get_info(arena_num)");
         for (int a = 0; a < A_; ++a) ib[a] = count(group, a);

@@ -258,6 +258,9 @@ private:
     void free_device();
     void *dalloc(size_t bytes);
     void *io_stage(size_t bytes);
+    // the per-agent read-backs (engine.cc read_back): one caller buffer (nullptr: not wanted) and its size in bytes
+    struct OutPart { void *buf; size_t bytes; };
+    template <size_t N, class F> void read_back(bool dev, const OutPart (&parts)[N], F &&launch);
     void stage_reserve(void *&p, size_t &have, size_t need);
     void get_observation_wire(int group, void **bufs);
     int max_agents_per_arena() const;

@@ -32,6 +32,29 @@ def _cint(v):
     return ctypes.byref(ctypes.c_int(int(v)))
 
 
+def _dptr(t):
+    """a tensor's data for the ABI; None (NULL) for None or an empty tensor, which has nothing to receive"""
+    return None if t is None or t.numel() == 0 else ctypes.c_void_p(t.data_ptr())
+
+
+def _check_cuda_out(t, what, dtypes, rows=None, tail=(), shape=None, align=1, optional=False):
+    """raise ValueError unless `t` is a contiguous CUDA tensor of one of `dtypes`, `align`-byte aligned, of exactly
+    `shape` or else of shape (r,) + tail with r >= rows.  optional: None is accepted too."""
+    import torch
+    if t is None and optional:
+        return
+    ok = (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype in dtypes and t.is_contiguous() and
+          t.data_ptr() % align == 0)
+    if ok:
+        s = tuple(t.shape)
+        ok = s == tuple(shape) if shape is not None else (len(s) == 1 + len(tail) and s[0] >= rows and s[1:] == tail)
+    if not ok:
+        want = (str(tuple(shape)) if shape is not None else
+                "(rows%s) with at least %d rows" % ("".join(", %d" % d for d in tail) or ",", rows))
+        raise ValueError("%s must be a contiguous%s CUDA tensor of dtype %s and shape %s" % (
+            what, ", %d-byte aligned" % align if align > 1 else "", " or ".join(map(str, dtypes)), want))
+
+
 class _HostBlock:
     """A growable host buffer; page-locked when the engine offers an allocator."""
 
@@ -246,13 +269,16 @@ class GridWorld(Environment):
         self.obs_bufs = [{}, {}, {}, {}]       # view, feature (reference); f16 view, f16 feature (extension)
         self._blocks = {}
 
+    def _host_view(self, key, shape, dtype):
+        """the cached receive buffer `key` as an array of `shape`: valid until the next call with the same key"""
+        block = self._blocks.get(key)
+        if block is None:
+            block = self._blocks[key] = _HostBlock(self._lib)
+        return block.view(shape, dtype)
+
     def _get_obs_buf(self, group, key, shape, dtype):
         """cached receive buffer, resized in place like the reference (gridworld.py:203-213)"""
-        block = self._blocks.get((group, key))
-        if block is None:
-            block = self._blocks[(group, key)] = _HostBlock(self._lib)
-        buf = block.view(shape, dtype)
-        self.obs_bufs[key][group] = buf
+        buf = self.obs_bufs[key][group] = self._host_view((group, key), shape, dtype)
         return buf
 
     def get_observation(self, handle):
@@ -470,15 +496,9 @@ class GridWorld(Environment):
         Per map cell: channel 0 wall, channel 1 food (food_mode only), then per group g in absolute order
         base + 2g presence and base + 2g + 1 hp / max_hp (base = 1 + food_mode); 0 elsewhere.  Every value equals
         the one a view covering the cell shows.  The array is a cached receive buffer: valid until the next call."""
-        buf = self._get_state_buf((self.num_arenas,) + self.get_state_space())
+        buf = self._host_view("state", (self.num_arenas,) + self.get_state_space(), np.float32)
         self._lib.magent_b200_get_global_state(self.game, buf.ctypes.data, 0)
         return buf
-
-    def _get_state_buf(self, shape):
-        block = self._blocks.get("state")
-        if block is None:
-            block = self._blocks["state"] = _HostBlock(self._lib)
-        return block.view(shape, np.float32)
 
     def get_global_state_torch(self, out=None, dtype=None):
         """the global state (see get_global_state) written straight into a CUDA tensor (num_arenas, H, W, C).
@@ -492,10 +512,7 @@ class GridWorld(Environment):
             out = torch.empty(shape, dtype=torch.float32 if dtype is None else dtype, device="cuda")
         elif dtype is not None and out.dtype != dtype:
             raise ValueError("out has dtype %s, not %s" % (out.dtype, dtype))
-        if out.dtype not in (torch.float32, torch.float16):
-            raise ValueError("global state dtype must be torch.float32 or torch.float16")
-        if (not out.is_cuda or tuple(out.shape) != shape or not out.is_contiguous() or out.data_ptr() % 16):
-            raise ValueError("out must be a contiguous, 16-byte aligned CUDA tensor of shape %s" % (shape,))
+        _check_cuda_out(out, "out", (torch.float32, torch.float16), shape=shape, align=16)
         self._lib.magent_b200_get_global_state(self.game, ctypes.c_void_p(out.data_ptr()),
                                                1 if out.dtype == torch.float16 else 0)
         return out
@@ -528,10 +545,7 @@ class GridWorld(Environment):
             ptr = src.ctypes.data
         else:
             import torch
-            if (not isinstance(src, torch.Tensor) or not src.is_cuda or src.dtype != torch.int32 or
-                    tuple(src.shape) != (self.num_arenas,) or not src.is_contiguous()):
-                raise ValueError("src must be an int32 numpy array or a contiguous int32 CUDA tensor of shape (%d,)"
-                                 % self.num_arenas)
+            _check_cuda_out(src, "src (when not an int32 numpy array)", (torch.int32,), shape=(self.num_arenas,))
             ptr = src.data_ptr()
         self._check(self._lib.magent_b200_restore_arenas(self.game, int(snapshot), ptr, 1 if keep_rng else 0),
                     "restore_arenas")
@@ -541,9 +555,7 @@ class GridWorld(Environment):
         import torch
         if out is None:
             out = torch.empty((self.num_arenas,), dtype=torch.int32, device="cuda")
-        if (not out.is_cuda or out.dtype != torch.int32 or tuple(out.shape) != (self.num_arenas,)
-                or not out.is_contiguous()):
-            raise ValueError("out must be a contiguous int32 CUDA tensor of shape (%d,)" % self.num_arenas)
+        _check_cuda_out(out, "out", (torch.int32,), shape=(self.num_arenas,))
         self._check(self._lib.magent_b200_get_arena_done(self.game, out.data_ptr()), "get_arena_done")
         return out
 
@@ -570,10 +582,7 @@ class GridWorld(Environment):
         set_action; a dead, un-culled agent's row is all False.  The array is a cached receive buffer: valid until the
         next call."""
         g = self._hv(handle)
-        block = self._blocks.get((g, "mask"))
-        if block is None:
-            block = self._blocks[(g, "mask")] = _HostBlock(self._lib)
-        buf = block.view((self.get_num(handle), self.action_space[g][0]), np.uint8)
+        buf = self._host_view((g, "mask"), (self.get_num(handle), self.action_space[g][0]), np.uint8)
         self._check(self._lib.magent_b200_get_action_mask(self.game, g, buf.ctypes.data), "get_action_mask")
         return buf.view(np.bool_)
 
@@ -591,11 +600,7 @@ class GridWorld(Environment):
         if out is None:
             out = torch.empty((n, na), dtype=torch.uint8, device="cuda")
         else:
-            if not isinstance(out, torch.Tensor) or not out.is_cuda or out.dtype not in (torch.bool, torch.uint8):
-                raise ValueError("out must be a CUDA tensor of dtype torch.bool or torch.uint8")
-            if out.dim() != 2 or out.shape[1] != na or not out.is_contiguous() or out.shape[0] < self.get_num_bound(handle):
-                raise ValueError("out must be contiguous, of shape (rows, %d) with at least %d rows"
-                                 % (na, self.get_num_bound(handle)))
+            _check_cuda_out(out, "out", (torch.bool, torch.uint8), rows=self.get_num_bound(handle), tail=(na,))
         self._check(self._lib.magent_b200_get_action_mask(self.game, g, ctypes.c_void_p(out.data_ptr())),
                     "get_action_mask")
         return out.view(torch.bool)[:n]
@@ -615,11 +620,8 @@ class GridWorld(Environment):
         g = self._hv(handle)
         o = g if of is None else self._hv(of)
         n = self.get_num(handle)
-        block = self._blocks.get((g, "mean"))
-        if block is None:
-            block = self._blocks[(g, "mean")] = _HostBlock(self._lib)
         na = self.action_space[o][0]
-        raw = block.view((n * (na + 1),), np.float32)
+        raw = self._host_view((g, "mean"), (n * (na + 1),), np.float32)
         mean, count = raw[:n * na].reshape(n, na), raw[n * na:].view(np.int32)
         self._check(self._lib.magent_b200_get_mean_action(self.game, g, o, mean.ctypes.data, count.ctypes.data),
                     "get_mean_action")
@@ -645,12 +647,8 @@ class GridWorld(Environment):
                 raise ValueError("out must be a (mean, count) pair of CUDA tensors")
             mean, count = out
             bound = self.get_num_bound(handle)
-            for t, dt, nd in ((mean, torch.float32, 2), (count, torch.int32, 1)):
-                if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dt:
-                    raise ValueError("out must be a CUDA float32 mean tensor and a CUDA int32 count tensor")
-                if t.dim() != nd or not t.is_contiguous() or t.shape[0] < bound or (nd == 2 and t.shape[1] != na):
-                    raise ValueError("out must be contiguous, of shapes (rows, %d) and (rows,) with at least %d rows"
-                                     % (na, bound))
+            _check_cuda_out(mean, "mean", (torch.float32,), rows=bound, tail=(na,))
+            _check_cuda_out(count, "count", (torch.int32,), rows=bound)
         self._check(self._lib.magent_b200_get_mean_action(self.game, g, o, ctypes.c_void_p(mean.data_ptr()),
                                                           ctypes.c_void_p(count.data_ptr())), "get_mean_action")
         return mean[:n], count[:n]
@@ -668,10 +666,7 @@ class GridWorld(Environment):
         if not 1 <= k <= 32:
             raise ValueError("k must be in [1, 32], got %d" % k)
         n = self.get_num(handle)
-        block = self._blocks.get((g, "nbr"))
-        if block is None:
-            block = self._blocks[(g, "nbr")] = _HostBlock(self._lib)
-        raw = block.view((n * (3 * k + 1),), np.int32)
+        raw = self._host_view((g, "nbr"), (n * (3 * k + 1),), np.int32)
         idx, rel, count = raw[:n * k].reshape(n, k), raw[n * k:3 * n * k].reshape(n, k, 2), raw[3 * n * k:]
         self._check(self._lib.magent_b200_get_neighbours(self.game, g, o, k, idx.ctypes.data, rel.ctypes.data,
                                                          count.ctypes.data), "get_neighbours")
@@ -702,18 +697,12 @@ class GridWorld(Environment):
                 raise ValueError("out must be an (idx, rel, count) triple of CUDA tensors")
             idx, rel, count = out
             bound = self.get_num_bound(handle)
-            for t, shape, opt in ((idx, (k,), False), (rel, (k, 2), True), (count, (), True)):
-                if t is None and opt:
-                    continue
-                if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.int32:
-                    raise ValueError("out must hold CUDA int32 tensors (rel and count may be None)")
-                if t.dim() != 1 + len(shape) or not t.is_contiguous() or t.shape[0] < bound or tuple(t.shape[1:]) != shape:
-                    raise ValueError("out must be contiguous, of shapes (rows, %d), (rows, %d, 2) and (rows,) with at "
-                                     "least %d rows" % (k, k, bound))
+            _check_cuda_out(idx, "idx", (torch.int32,), rows=bound, tail=(k,))
+            _check_cuda_out(rel, "rel", (torch.int32,), rows=bound, tail=(k, 2), optional=True)
+            _check_cuda_out(count, "count", (torch.int32,), rows=bound, optional=True)
         if idx.shape[0] == 0:            # no row can be written (num_bound is 0), and an empty tensor's pointer is NULL
             return idx, rel, count
-        ptr = (lambda t: None if t is None else ctypes.c_void_p(t.data_ptr()))
-        self._check(self._lib.magent_b200_get_neighbours(self.game, g, o, k, ptr(idx), ptr(rel), ptr(count)),
+        self._check(self._lib.magent_b200_get_neighbours(self.game, g, o, k, _dptr(idx), _dptr(rel), _dptr(count)),
                     "get_neighbours")
         return idx[:n], None if rel is None else rel[:n], None if count is None else count[:n]
 
@@ -735,10 +724,7 @@ class GridWorld(Environment):
         n = self.get_num(handle)                 # settles the counts, so the bound below is the call's
         bound = self.get_num_bound(handle)
         S = self.get_slot_space(handle)
-        block = self._blocks.get((g, "slots"))
-        if block is None:
-            block = self._blocks[(g, "slots")] = _HostBlock(self._lib)
-        raw = block.view((bound + self.num_arenas * S,), np.int32)
+        raw = self._host_view((g, "slots"), (bound + self.num_arenas * S,), np.int32)
         row_slot, slot_row = raw[:bound], raw[bound:].reshape(self.num_arenas, S)
         self._check(self._lib.magent_b200_get_slots(self.game, g, row_slot.ctypes.data, slot_row.ctypes.data),
                     "get_slots")
@@ -766,19 +752,11 @@ class GridWorld(Environment):
             if not isinstance(out, (tuple, list)) or len(out) != 2 or (out[0] is None and out[1] is None):
                 raise ValueError("out must be a (row_slot, slot_row) pair of CUDA tensors, at most one of them None")
             row_slot, slot_row = out
-            for t in (row_slot, slot_row):
-                if t is not None and (not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.int32 or
-                                      not t.is_contiguous()):
-                    raise ValueError("out must hold contiguous CUDA int32 tensors")
-            if row_slot is not None and (row_slot.dim() != 1 or row_slot.shape[0] < bound):
-                raise ValueError("row_slot must be of shape (rows,) with at least %d rows" % bound)
-            if slot_row is not None and tuple(slot_row.shape) != (self.num_arenas, S):
-                raise ValueError("slot_row must be of shape (%d, %d)" % (self.num_arenas, S))
-        # an empty tensor's pointer is NULL: it has nothing to receive
-        ptr = (lambda t: None if t is None or t.numel() == 0 else ctypes.c_void_p(t.data_ptr()))
-        if ptr(row_slot) is None and ptr(slot_row) is None:
+            _check_cuda_out(row_slot, "row_slot", (torch.int32,), rows=bound, optional=True)
+            _check_cuda_out(slot_row, "slot_row", (torch.int32,), shape=(self.num_arenas, S), optional=True)
+        if _dptr(row_slot) is None and _dptr(slot_row) is None:
             return row_slot, slot_row
-        self._check(self._lib.magent_b200_get_slots(self.game, g, ptr(row_slot), ptr(slot_row)), "get_slots")
+        self._check(self._lib.magent_b200_get_slots(self.game, g, _dptr(row_slot), _dptr(slot_row)), "get_slots")
         return row_slot, slot_row
 
     def get_counters(self):
