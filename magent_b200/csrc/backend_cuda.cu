@@ -78,6 +78,7 @@ struct Ctx {
     // cudaFuncSetAttribute caches (per device: a context never changes device)
     struct ObsCfg { size_t smem = (size_t)-1; int ctas_per_sm = 1; } obs_cfg[12];
     int obs_last[8] = {0, 0, 0, 0, 0, 0, 0, 0};            // the last render launch (obs_launch_report)
+    unsigned *obs_deal = nullptr;        // [sms + 1] render chunk counters; zero between launches (the kernel resets them)
     ObsCfg state_cfg[2];                 // global_state_kernel<float>, <__half>: CTAs per SM (smem 0 once queried)
     int restore_ctas_per_sm = 0;         // restore_kernel (0: not queried yet)
     int *pin_done = nullptr; size_t pin_done_n = 0;         // pinned read-back of EngineDev::done
@@ -144,6 +145,8 @@ Ctx *create(int device, std::string *err) {
     CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_wire, cudaEventDisableTiming));
     CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming));
     CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_counts, cudaEventDisableTiming));
+    CUDA_CHECK(cudaMalloc(&c->obs_deal, (c->sms + 1) * sizeof(unsigned)));
+    CUDA_CHECK(cudaMemset(c->obs_deal, 0, (c->sms + 1) * sizeof(unsigned)));
     return c;
 }
 void destroy(Ctx *c) {
@@ -155,7 +158,7 @@ void destroy(Ctx *c) {
     for (cudaEvent_t e : c->wave_events) cudaEventDestroy(e);
     for (cudaEvent_t e : c->dma_events) cudaEventDestroy(e);
     cudaEventDestroy(c->ev_wire); cudaEventDestroy(c->ev_done);
-    cudaFree(c->mm_pad); cudaFree(c->obs_hdr);
+    cudaFree(c->mm_pad); cudaFree(c->obs_hdr); cudaFree(c->obs_deal);
     cudaFree(c->wire_slots); cudaFree(c->wire_stream); cudaFree(c->wire_hdr); cudaFree(c->wire_base); cudaFree(c->wire_chunk_total);
     cudaEventDestroy(c->ev_counts); cudaFreeHost(c->pin_counts);
     cudaFreeHost(c->pin_done); cudaFreeHost(c->h_wire_hdr); cudaFreeHost(c->h_wire_marks); cudaFreeHost(c->h_wire_base); cudaFreeHost(c->h_mm);
@@ -1178,8 +1181,10 @@ void launch_obs_prepare(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsign
 // throughput summed over reads and writes -- so every byte the kernel READS through L2 competes with the bytes it
 // writes:
 //   * tile = TA consecutive agents of the ABI concatenation = ONE CTA of TA warps, one warp per agent, one
-//     shared-memory tile, 32 warps per SM (battle f32: 8 agents, 37.9 KB, 4 CTAs per SM), tiles dealt round-robin so
-//     the whole grid works inside a window of a few arenas (their planes / minimaps stay L1/L2-hot);
+//     shared-memory tile, 32 warps per SM (battle f32: 8 agents, 37.9 KB, 4 CTAs per SM), chunks of tiles dealt per
+//     SM through device counters, so the CTAs of one SM compose neighbouring observers of one arena together (its
+//     plane rows are shared in L1) and the whole grid works inside a window of a few arenas (planes / minimaps
+//     L2-hot);
 //   * the map is gathered from a ONE-BYTE kind plane (0 empty / 1 wall / 2+group; a view row is one 32-byte
 //     sector) and only occupied cells (~5 %) take a second, dependent load from the hp_norm plane;
 //   * the tile is composed entirely on the SM: each warp zero-fills its own record, copies the arena's
@@ -1230,6 +1235,9 @@ struct ObsParams {
     int kpad, kw;
     long kplane;
     int chunk;                       // consecutive tiles per CTA visit (<= OBS_CHUNK)
+    unsigned *deal;                  // [sms + 1] chunk counters per SM + done counter (Ctx::obs_deal), or nullptr:
+                                     // chunks round-robin over the CTAs
+    int sms, deal_unit;              // the SMs that own chunk sequences; chunks per unit of a sequence
     int turn, body_w, body_l;        // turn_mode: 4 view LUTs (one per heading), the heading rides in the header
     const unsigned char *dir;
     const int *x, *y, *id, *act;
@@ -1310,7 +1318,13 @@ __global__ void __launch_bounds__(256) obs_headers_kernel(ObsParams P, int4 *hdr
 template <typename T> constexpr int obs_tile_narrow() { return 16 / (int)sizeof(T); }
 template <typename T> constexpr int obs_tile_wide() { return 32 / (int)sizeof(T); }
 #ifndef OBS_CHUNK
-#define OBS_CHUNK 4                  // consecutive tiles a CTA renders before it jumps ahead by grid * OBS_CHUNK tiles
+#define OBS_CHUNK 4                  // consecutive tiles a CTA renders before it claims its next chunk
+#endif
+#ifndef OBS_DEAL_UNIT
+#define OBS_DEAL_UNIT 4              // a unit of an SM's chunk sequence = OBS_DEAL_UNIT * (CTAs per SM) consecutive chunks
+#endif
+#ifndef OBS_DEAL_MIN_UNITS
+#define OBS_DEAL_MIN_UNITS 4         // automatic launches deal per SM only with at least this many units per SM
 #endif
 // NIT = view cells per lane held in registers (NIT * 32 >= in-range cells of the view whenever that is <= 256;
 // larger views take the unpipelined tail loop).
@@ -1338,7 +1352,82 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
     // padded planes relative to the observer's own cell}
     int2 *lut = (int2 *)(buf + OBS_TA * P.rec);
     __shared__ int n_in_s;
+    __shared__ int deal_s[4];                                 // claimed tiles: the first three, then the next chunk's start
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int n_tiles = (n_total + OBS_TA - 1) / OBS_TA;
+
+    // Tile assignment: chunks of P.chunk consecutive tiles; within a chunk the arena (almost) never changes, so the
+    // persistent tile needs no rebuild.  With P.deal, the chunks are dealt per SM: units of P.deal_unit consecutive
+    // chunks go round-robin to the SMs, and SM s's sequence of units is handed out chunk by chunk by counter s.  Every
+    // CTA resident on SM s claims from counter s, so the CTAs of one SM compose neighbouring observers of one arena at
+    // the same time and share its kind / hp plane rows in L1; all SMs still advance together through the output, inside
+    // a window of about sms * unit chunks (a blocked assignment -- one contiguous region per CTA -- would spread the
+    // stream over the whole output, beyond the TLB reach).  A CTA whose SM's sequence is drained claims from the other
+    // counters in the order home + 1, home + 2, ..., so every chunk is rendered exactly once whatever the placement
+    // of the CTAs (an SM without CTAs, an SM with more than the occupancy, a forced grid of 1), and the CTAs finish
+    // together.  Without P.deal (a single round, or too few units per SM: launch_obs_render) the chunks go round-robin
+    // over the CTAs: CTA b renders chunks b, b + grid, b + 2 * grid, ...
+    // Warp 0 claims; a claim returns the first tile of the claimed chunk, n_tiles when there is none left.  The claim
+    // of the chunk that follows tile i+2 is issued before tile i is composed and read after it (CLAIM_LATE), or before
+    // it for the float NIT = 8 instantiations: they have no register to spare across the composition (holding the
+    // claim there cost them 60 bytes of spills per thread).
+    constexpr bool CLAIM_LATE = !(sizeof(T) == 4 && NIT == 8);
+    const int chunk = P.chunk;
+    // warp 0's claim state, in shared memory so that it holds no register across the tile loop: this CTA's SM (its
+    // home counter; %smid need not be dense, and any counter is correct) and the counters drained so far, in the
+    // order home, home + 1, ...
+    __shared__ int home_s, drained_s;
+    if (threadIdx.x == 0 && P.deal) {
+        unsigned smid;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+        home_s = (int)(smid % (unsigned)P.sms);
+        drained_s = 0;
+    }
+    __syncwarp();
+    auto seq_chunk = [&](int s, unsigned j, int n_chunks) -> int {   // chunk j of SM s's sequence (n_chunks: beyond its end)
+        const long c = ((long)(j / P.deal_unit) * P.sms + s) * P.deal_unit + j % P.deal_unit;
+        return c < n_chunks ? (int)c : n_chunks;
+    };
+    auto counter_of = [&](int home, int drained) -> int { return home + drained < P.sms ? home + drained : home + drained - P.sms; };
+    // lane 0 of warp 0 takes a chunk index from the counter being drained; the atomic is issued ahead of claim() so
+    // that its latency hides behind other work
+    auto issue_claim = [&]() -> unsigned {
+        return lane == 0 && drained_s < P.sms ? atomicAdd(P.deal + counter_of(home_s, drained_s), 1u) : 0u;
+    };
+    // warp 0, warp-uniform, P.deal only: the first tile of the claimed chunk (j = issue_claim()), n_tiles when none is left
+    auto claim = [&](unsigned j) -> int {
+        const int n_chunks = (n_tiles + chunk - 1) / chunk;
+        const int home = home_s;
+        int drained = drained_s, tile = n_tiles;
+        __syncwarp();
+        while (drained < P.sms) {
+            const int c = __shfl_sync(0xffffffffu, lane == 0 ? seq_chunk(counter_of(home, drained), j, n_chunks) : 0, 0);
+            if (c < n_chunks) { tile = c * chunk; break; }
+            int next = P.sms;                             // this counter is drained: find the next live one, 32 at a time
+            for (int base = drained + 1; base < P.sms; base += 32) {
+                const int s = counter_of(home, base + lane);
+                unsigned js = 0;
+                if (base + lane < P.sms) asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(js) : "l"(P.deal + s) : "memory");
+                const unsigned b = __ballot_sync(0xffffffffu, base + lane < P.sms && seq_chunk(s, js, n_chunks) < n_chunks);
+                if (b) { next = base + __ffs(b) - 1; break; }
+            }
+            drained = next;
+            if (drained < P.sms && lane == 0) j = atomicAdd(P.deal + counter_of(home, drained), 1u);
+        }
+        if (lane == 0) drained_s = drained;
+        __syncwarp();
+        return tile;
+    };
+    // the tile after t: t + 1 inside its chunk, else nxt (the next claimed chunk) or the CTA's next round-robin chunk;
+    // n_tiles past the end
+    auto ends_chunk = [&](int t) -> bool { return t < n_tiles && (t + 1 == n_tiles || (t + 1) % chunk == 0); };
+    auto next_tile = [&](int t, bool ends, int nxt) -> int {          // ends = ends_chunk(t)
+        if (t >= n_tiles) return n_tiles;
+        if (!ends) return t + 1;
+        if (P.deal) return nxt;
+        const long r = (long)t + 1 + (long)(gridDim.x - 1) * chunk;
+        return r < n_tiles ? (int)r : n_tiles;
+    };
 
     const int lut_stride = (P.cells + 1) & ~1;
     if (warp == 0) {                                          // compact the view mask (Range.h:104-189)
@@ -1370,10 +1459,15 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
             k += __popc(bal);
         }
         if (lane == 0) n_in_s = k;
+        if (P.deal) {                                         // the pipeline starts with three tiles: claim their chunks
+            const int t0 = claim(issue_claim());
+            const int t1 = ends_chunk(t0) ? claim(issue_claim()) : next_tile(t0, false, n_tiles);
+            const int t2 = ends_chunk(t1) ? claim(issue_claim()) : next_tile(t1, false, n_tiles);
+            if (lane == 0) { deal_s[0] = t0; deal_s[1] = t1; deal_s[2] = t2; }
+        }
     }
     __syncthreads();
     const int n_in = n_in_s;
-    const int n_tiles = (n_total + OBS_TA - 1) / OBS_TA;
     // this lane's slice of the view LUT never changes: small views keep it in registers, large ones re-read smem
     constexpr bool LUT_REGS = obs_all_cells_in_regs<NIT, TURN>();
     int2 lreg[LUT_REGS ? NIT : 1];
@@ -1424,17 +1518,11 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
         if (agent) px[ch + 1] = ObsOut<T>::cv(on ? hp : 0.0f);             // hp / max_hp (Map.cc:197)
     };
 
-    // tile assignment: chunks of OBS_CHUNK consecutive tiles, dealt round-robin over the CTAs.  Inside a chunk the
-    // arena (almost) never changes, so the persistent tile needs no rebuild; across the grid all CTAs write inside one
-    // window of grid * OBS_CHUNK tiles (~80 MB on H100), which keeps the output stream inside the TLB reach (a
-    // blocked assignment -- one contiguous region per CTA -- would spread it over the whole output) and the planes of
-    // ~20 arenas L2-hot.
-    // Software pipeline: while tile i is composed, the kind loads of tile i+1 and the header load of tile i+2 fly.
-    const int chunk = P.chunk;                 // 1 when there are too few tiles to keep every CTA busy with longer chunks
-    const int chunk_jump = ((int)gridDim.x - 1) * chunk;
-    auto next_tile = [&](int t) -> int { return ((t + 1) % chunk) ? t + 1 : t + 1 + chunk_jump; };
-    int tile = blockIdx.x * chunk;
-    int tile1 = next_tile(tile), tile2 = next_tile(tile1);
+    // Software pipeline: while tile i is composed, the kind loads of tile i+1 and the header load of tile i+2 fly; the
+    // chunk that follows tile i+2 is claimed during tile i and passed on at one of its barriers.
+    int tile = (int)blockIdx.x < (n_tiles + chunk - 1) / chunk ? (int)blockIdx.x * chunk : n_tiles;
+    int tile1 = next_tile(tile, ends_chunk(tile), n_tiles), tile2 = next_tile(tile1, ends_chunk(tile1), n_tiles);
+    if (P.deal) { tile = deal_s[0]; tile1 = deal_s[1]; tile2 = deal_s[2]; }
     const int tile_end = n_tiles;
     const int4 zero4 = make_int4(0, 0, 0, 0);
     int4 hA = zero4, hA1 = zero4;             // headers of tile i and i+1
@@ -1455,7 +1543,7 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
         if (o1 < n_total) hA1 = P.hdr[o1];
         load_kinds(hA, on0, kind);
     }
-    for (; tile < tile_end; tile = tile1, tile1 = tile2, tile2 = next_tile(tile2)) {
+    for (int tile3; tile < tile_end; tile = tile1, tile1 = tile2, tile2 = tile3) {
         const int t0 = tile * OBS_TA;
         const int cnt = min(OBS_TA, n_total - t0);
         const bool active = warp < cnt;
@@ -1481,9 +1569,16 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
         }
         // the previous tile's bulk store must have finished READING the buffer before it is touched.  One buffer per
         // CTA on purpose: a second would cost a CTA per SM, and at battle's size that loses more than the overlap
-        // wins (DESIGN.md section 5, "Two tile slots per CTA")
+        // wins (DESIGN.md section 5, "Two tile slots per CTA").  The claim's atomic flies while the tile is composed.
+        const bool ends2 = ends_chunk(tile2), claims = P.deal && ends2;
+        const unsigned j = claims && warp == 0 ? issue_claim() : 0u;
         if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        if (!CLAIM_LATE && claims && warp == 0) {
+            const int t = claim(j);
+            if (lane == 0) deal_s[3] = t;
+        }
         __syncthreads();
+        if (!CLAIM_LATE) tile3 = next_tile(tile2, ends2, claims ? deal_s[3] : n_tiles);   // read before the next barrier
         if (active && !(OBS_ABLATE & 2)) {
             T *dst = buf + warp * P.rec;
             const int self = (int)(short)(hA.w & 0xffff);
@@ -1558,9 +1653,14 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
                 prev_tail = true;
             }
         }
+        if (CLAIM_LATE && claims && warp == 0) {
+            const int t = claim(j);
+            if (lane == 0) deal_s[3] = t;
+        }
         // make the generic-proxy writes visible to the async proxy, then one thread fires the bulk store
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
+        if (CLAIM_LATE) tile3 = next_tile(tile2, ends2, claims ? deal_s[3] : n_tiles);   // read before the next barrier: deal_s[3] is rewritten after it
         T *gout = (T *)P.view + (size_t)t0 * P.rec;
         const unsigned bytes = (unsigned)cnt * (unsigned)P.rec * (unsigned)sizeof(T);
         if ((bytes & 15u) == 0 && (((size_t)gout) & 15) == 0) {
@@ -1583,7 +1683,14 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
 #pragma unroll
         for (int q = 0; q < KW; ++q) kind[q] = kind1[q];
     }
-    if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    if (threadIdx.x == 0) {
+        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+        if (P.deal) {                          // the last CTA to finish (every claim is made) zeroes the counters for
+            __threadfence();                   // the next launch: a replayed graph needs no memset node
+            if (atomicAdd(P.deal + P.sms, 1u) == gridDim.x - 1)
+                for (int s = 0; s <= P.sms; ++s) P.deal[s] = 0u;
+        }
+    }
 }
 
 // CTAs per SM of one render instantiation at this shared-memory size (0: it does not fit), cached per context slot
@@ -1600,8 +1707,8 @@ static int obs_ctas_per_sm(Ctx *c, int cfg_slot, size_t smem) {
 }
 
 // O.grid / O.chunk > 0 replace the automatic grid and chunk (tests: CTAs that render many tiles at small sizes).
-// Both are clamped: grid to [1, tiles], chunk to [1, ceil(tiles / grid)], so that the kernel's tile indices, up to
-// (grid - 1) * chunk past a tile it renders, stay far from int overflow.  The clamps never change the automatic values.
+// Both are clamped: grid to [1, tiles], chunk to [1, ceil(tiles / grid)], so that no CTA is launched without a tile
+// and no chunk is longer than a CTA's share.  The clamps never change the automatic values.
 template <typename T, int NIT, bool TURN, int TA>
 static void launch_obs_render(Ctx *c, const ObsArgs &O, ObsParams &P, int n_total, size_t smem, int ctas_per_sm) {
     const int g_sms = c->sms;
@@ -1615,6 +1722,15 @@ static void launch_obs_render(Ctx *c, const ObsArgs &O, ObsParams &P, int n_tota
     if (O.chunk > 0) P.chunk = O.chunk;
     grid = std::max(1, std::min(grid, tiles));
     P.chunk = std::max(1, std::min(P.chunk, (tiles + grid - 1) / grid));
+    // more than one round of chunks: deal them per SM (obs_render_kernel) when every SM owns at least
+    // OBS_DEAL_MIN_UNITS units, or when the grid is forced (tests: the claims and the stealing at small sizes);
+    // otherwise round-robin.  With fewer units per SM the deal measured slower (DESIGN.md section 5, "Chunks dealt
+    // per SM"): battle512 in float16 at 3.8 units per SM, gather64 at under 2.
+    P.sms = g_sms;
+    P.deal_unit = OBS_DEAL_UNIT * ctas_per_sm;
+    const long chunks = (tiles + P.chunk - 1) / P.chunk;
+    const bool rounds = (long)grid * P.chunk < tiles;
+    P.deal = rounds && (O.grid > 0 || chunks >= (long)OBS_DEAL_MIN_UNITS * P.deal_unit * g_sms) ? c->obs_deal : nullptr;
     const int aligned = ((((size_t)P.view) | ((size_t)P.feature)) & 15) == 0;
     const int report[8] = {(int)sizeof(T), NIT, TURN ? 1 : 0, TA, grid, P.chunk, tiles, aligned};
     memcpy(c->obs_last, report, sizeof report);
