@@ -113,6 +113,20 @@ int magent_b200_get_neighbours(EnvHandle game, GroupHandle group, GroupHandle of
  * pointers, pointers that mix host and CUDA device memory, or a backend without the kernel.  magent_b200_select_arena
  * does not apply. */
 int magent_b200_get_slots(EnvHandle game, GroupHandle group, int *row_slot, int *slot_row);
+/* the observation of one group in the stable [arena, slot] layout of magent_b200_get_slots, rendered in that order:
+ *   buffer[0] = view [num_arenas][S][view_h][view_w][n_channel], buffer[1] = feature [num_arenas][S][feature_size],
+ *   S = env_get_info(game, -1, "slot_space", int[n_group])[group].
+ * An occupied slot (a, s) holds, bit for bit, the view record and feature row env_get_observation (half = 1:
+ * magent_b200_get_observation_f16) writes at the same moment for row slot_row[a][s]; a dead agent that has not been culled
+ * keeps its slot and its record.  A vacant slot holds an all-zero view record and feature row (+0.0).  half = 0:
+ * float32; half = 1: IEEE binary16, the float32 value rounded to nearest-even.  Covers every arena whatever
+ * magent_b200_select_arena says; S == 0 writes nothing.  Both CUDA device pointers: no synchronisation and, once a
+ * first call has sized the engine's tables, no allocation, so the call can be recorded into a CUDA graph, also after a
+ * restore from a device src inside the graph (the device decides which slots hold rows).  Both host pointers: rendered
+ * into device staging and copied back (counted in the d2h figure of magent_b200_get_io_stats).  Returns -1, sets
+ * magent_b200_last_error and writes nothing for a bad group handle, half other than 0 or 1, a NULL pointer, pointers that
+ * mix host and CUDA device memory, or a backend without the kernel. */
+int magent_b200_get_observation_slots(EnvHandle game, GroupHandle group, void **buffer, int half);
 /* compact observation hand-off (SURVEY.md 8f rank 2): same call, layout and pointer rules as env_get_observation
  * (reference src/runtime_api.h:35), but every element is an IEEE binary16 = the float32 value rounded to
  * nearest-even.  buffer[0] = view [n][view_h][view_w][n_channel], buffer[1] = feature [n][feature_size];

@@ -104,6 +104,13 @@ __attribute__((weak)) void launch_slots(Ctx *, const EngineDev *dE, const Engine
                                         unsigned curmask, int group, int S, int *row_slot, int *slot_row, int n_bound);
 __attribute__((weak)) void launch_restore_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
                                                 const int *snap_tab, int snap_id_cap, const int *src);
+// Observation O of group O.group in slot order (magent_b200_get_observation_slots): O.view [A][S] records and O.feature
+// [A][S] rows, both device buffers; record a * S + s is the one launch_obs writes for the row in slot s of arena a
+// (slot_phases.h, the device-side offsets decide the rows), all zeros where no row is.  mm_val as for launch_obs (the
+// engine ran launch_obs_prepare for this group).  The kind plane must be followed by the blank window of
+// EngineDev::kind.  Weak like launch_slots: the engine refuses the call without it.
+__attribute__((weak)) void launch_obs_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
+                                            const ObsArgs &O, const float *mm_val, int S);
 // clear_dead: asynchronous read-back of the [G][A+1] offset table (launch_offsets) into page-locked memory
 void counts_fetch_begin(Ctx *, const int *dev_off, size_t n_ints);
 const int *counts_fetch_wait(Ctx *);     // blocks until the fetch has landed; valid until the next counts_fetch_begin

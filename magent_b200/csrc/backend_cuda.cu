@@ -75,6 +75,10 @@ struct Ctx {
     float *mm_pad = nullptr; size_t mm_pad_n = 0; int mm_stride = 0;
     // per-observer headers of the render kernel
     int4 *obs_hdr = nullptr; size_t obs_hdr_n = 0;
+    // slot-ordered observations (launch_obs_slots): the [A][S] slot -> row scratch, and the render's count bound
+    // ([A + 1] words of INT_MAX)
+    int *obs_slot_row = nullptr; size_t obs_slot_row_n = 0;
+    int *obs_slot_bound = nullptr; size_t obs_slot_bound_n = 0;
     // cudaFuncSetAttribute caches (per device: a context never changes device)
     struct ObsCfg { size_t smem = (size_t)-1; int ctas_per_sm = 1; } obs_cfg[12];
     int obs_last[8] = {0, 0, 0, 0, 0, 0, 0, 0};            // the last render launch (obs_launch_report)
@@ -158,7 +162,7 @@ void destroy(Ctx *c) {
     for (cudaEvent_t e : c->wave_events) cudaEventDestroy(e);
     for (cudaEvent_t e : c->dma_events) cudaEventDestroy(e);
     cudaEventDestroy(c->ev_wire); cudaEventDestroy(c->ev_done);
-    cudaFree(c->mm_pad); cudaFree(c->obs_hdr); cudaFree(c->obs_deal);
+    cudaFree(c->mm_pad); cudaFree(c->obs_hdr); cudaFree(c->obs_deal); cudaFree(c->obs_slot_row); cudaFree(c->obs_slot_bound);
     cudaFree(c->wire_slots); cudaFree(c->wire_stream); cudaFree(c->wire_hdr); cudaFree(c->wire_base); cudaFree(c->wire_chunk_total);
     cudaEventDestroy(c->ev_counts); cudaFreeHost(c->pin_counts);
     cudaFreeHost(c->pin_done); cudaFreeHost(c->h_wire_hdr); cudaFreeHost(c->h_wire_marks); cudaFreeHost(c->h_wire_base); cudaFreeHost(c->h_mm);
@@ -1148,7 +1152,7 @@ void launch_obs_prepare(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsign
     int cap_max = 0;
     for (int g = 0; g < hE.G; ++g) cap_max = cap_max > hE.grp[g].cap ? cap_max : hE.grp[g].cap;
     c->mm_stride = (hE.G * cells + 3) & ~3;
-    const size_t need = (size_t)hE.A * c->mm_stride;
+    const size_t need = (size_t)(hE.A + 1) * c->mm_stride;         // row A: the blank arena's (launch_obs_slots)
     if (need > c->mm_pad_n) {
         no_capture(c, "growing the minimap buffer");
         if (c->mm_pad) { CUDA_CHECK(cudaStreamSynchronize(c->stream)); CUDA_CHECK(cudaStreamSynchronize(c->copy)); cudaFree(c->mm_pad); }
@@ -1252,14 +1256,54 @@ struct ObsParams {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// pre-pass, one thread per observer, CTAs dealt per arena (no search for the arena: blockIdx says it):
+// One observer of the pre-passes, agent i of arena a: returns its render header and writes the non-zeros of its
+// feature row into f (F elements, zero-filled by the caller).
 //   * header h = {x, y, arena, self minimap cell | heading << 16}: everything the render kernel needs about the observer itself, so
 //     that its only dependent loads are kind plane -> hp_norm plane;
 //   * the complete non-spatial feature row (GridWorld.cc:386-396): id bits LSB first, one-hot last action, last
 //     reward, and x/W, y/H with the minimap.  A fresh agent's last_action == n_action ("dangerous", GridWorld.h:140)
-//     lands on the reward slot and is overwritten by it -- here the reward simply wins.  The rows of a CTA's observers are
-//     one contiguous block of the output: composed in shared memory (zero fill, then every thread its own handful of
-//     non-zeros), written out with coalesced stores.
+//     lands on the reward slot and is overwritten by it -- here the reward simply wins.
+template <typename T>
+__device__ __forceinline__ int4 obs_observer(const ObsParams &P, int a, int i, T *f) {
+    const long gi = (long)a * P.cap + i;
+    const int x = P.x[gi], y = P.y[gi];
+    const int self_cell = P.minimap ? (y / P.scale_h) * P.vw + x / P.scale_w : -1;  // GridWorld.cc:372-373
+    const int heading = P.turn ? (int)P.dir[gi] : 0;
+    unsigned id = (unsigned)P.id[gi];
+    const int nbits = min(P.embedding, 31);
+    id &= nbits >= 32 ? 0xffffffffu : ((1u << nbits) - 1u);
+    while (id) {                                           // embedding: the set bits of the id, LSB first (GridWorld.h:155-164)
+        const int bit = __ffs(id) - 1;
+        f[bit] = ObsOut<T>::cv(1.0f);
+        id &= id - 1;
+    }
+    T *g = f + P.embedding;
+    const int act = P.act[gi];
+    if (act >= 0 && act < P.n_action) g[act] = ObsOut<T>::cv(1.0f);
+    g[P.n_action] = ObsOut<T>::cv(P.last_reward[gi]);       // also overwrites the "dangerous" fresh-agent one-hot slot
+    if (P.minimap) {
+        g[P.n_action + 1] = ObsOut<T>::cv((float)x / (float)P.W);               // GridWorld.cc:394-395
+        g[P.n_action + 2] = ObsOut<T>::cv((float)y / (float)P.H);
+    }
+    return make_int4(x, y, a, (self_cell & 0xffff) | (heading << 16));
+}
+
+// the cnt * F elements of `rows` (shared memory) into out, coalesced
+template <typename T>
+__device__ __forceinline__ void obs_store_rows(T *out, const T *rows, int total) {
+    if (sizeof(T) == 4 && ((((size_t)out) & 15) == 0)) {       // 16-byte body, scalar tail
+        const int v4 = total >> 2;
+        for (int q = threadIdx.x; q < v4; q += blockDim.x) ((float4 *)out)[q] = ((const float4 *)rows)[q];
+        for (int q = (v4 << 2) + threadIdx.x; q < total; q += blockDim.x) out[q] = rows[q];
+    } else {
+        for (int q = threadIdx.x; q < total; q += blockDim.x) out[q] = rows[q];
+    }
+}
+
+// pre-pass, one thread per observer, CTAs dealt per arena (no search for the arena: blockIdx says it): the header and
+// feature row of every observer (obs_observer).  The rows of a CTA's observers are one contiguous block of the output:
+// composed in shared memory (zero fill, then every thread its own handful of non-zeros), written out with coalesced
+// stores.
 template <typename T>
 __global__ void __launch_bounds__(256) obs_headers_kernel(ObsParams P, int4 *hdr, int chunks_per_arena) {
     extern __shared__ __align__(16) unsigned char hdr_smem[];
@@ -1276,38 +1320,37 @@ __global__ void __launch_bounds__(256) obs_headers_kernel(ObsParams P, int4 *hdr
     __syncthreads();
     if ((int)threadIdx.x < cnt) {
         const int i = i0 + threadIdx.x;
-        const long gi = (long)a * P.cap + i;
-        const int x = P.x[gi], y = P.y[gi];
-        const int self_cell = P.minimap ? (y / P.scale_h) * P.vw + x / P.scale_w : -1;  // GridWorld.cc:372-373
-        const int heading = P.turn ? (int)P.dir[gi] : 0;
-        hdr[o0 + i] = make_int4(x, y, a, (self_cell & 0xffff) | (heading << 16));
-        T *f = rows + (size_t)threadIdx.x * P.F;
-        unsigned id = (unsigned)P.id[gi];
-        const int nbits = min(P.embedding, 31);
-        id &= nbits >= 32 ? 0xffffffffu : ((1u << nbits) - 1u);
-        while (id) {                                           // embedding: the set bits of the id, LSB first (GridWorld.h:155-164)
-            const int bit = __ffs(id) - 1;
-            f[bit] = ObsOut<T>::cv(1.0f);
-            id &= id - 1;
-        }
-        T *g = f + P.embedding;
-        const int act = P.act[gi];
-        if (act >= 0 && act < P.n_action) g[act] = ObsOut<T>::cv(1.0f);
-        g[P.n_action] = ObsOut<T>::cv(P.last_reward[gi]);       // also overwrites the "dangerous" fresh-agent one-hot slot
-        if (P.minimap) {
-            g[P.n_action + 1] = ObsOut<T>::cv((float)x / (float)P.W);               // GridWorld.cc:394-395
-            g[P.n_action + 2] = ObsOut<T>::cv((float)y / (float)P.H);
-        }
+        hdr[o0 + i] = obs_observer<T>(P, a, i, rows + (size_t)threadIdx.x * P.F);
     }
     __syncthreads();
-    T *out = (T *)P.feature + (size_t)(o0 + i0) * P.F;
-    if (sizeof(T) == 4 && ((((size_t)out) & 15) == 0)) {       // 16-byte body, scalar tail
-        const int v4 = total >> 2;
-        for (int q = threadIdx.x; q < v4; q += blockDim.x) ((float4 *)out)[q] = ((const float4 *)rows)[q];
-        for (int q = (v4 << 2) + threadIdx.x; q < total; q += blockDim.x) out[q] = rows[q];
-    } else {
-        for (int q = threadIdx.x; q < total; q += blockDim.x) out[q] = rows[q];
+    obs_store_rows<T>((T *)P.feature + (size_t)(o0 + i0) * P.F, rows, total);
+}
+
+// the slot-ordered pre-pass (magent_b200_get_observation_slots): the same header and feature row per slot, in [A][S]
+// order.  slot_row ([A][S], slots_kernel) names the row in each slot, -1 when vacant; `off` are the group's device-side
+// offsets (P.off is the render's count bound in a slot launch).  CTAs are dealt per arena, one thread per slot, so
+// every header and every feature row is written exactly once and the stores are coalesced whatever the slots' order.
+// A vacant slot gets the header of the blank arena A ({0, 0, A, 0}: see launch_obs_slots) and a zero feature row.
+template <typename T>
+__global__ void __launch_bounds__(256) obs_slot_headers_kernel(ObsParams P, const int *off, const int *slot_row, int S,
+                                                               int4 *hdr, int chunks_per_arena) {
+    extern __shared__ __align__(16) unsigned char hdr_smem[];
+    T *rows = (T *)hdr_smem;                                   // [blockDim.x][F]
+    const int a = blockIdx.x / chunks_per_arena;
+    const int s0 = (blockIdx.x - a * chunks_per_arena) * blockDim.x;
+    if (s0 >= S) return;
+    const int cnt = min((int)blockDim.x, S - s0);
+    const int total = cnt * P.F;
+    const long o = (long)a * S + s0;                           // first slot of this CTA in [A][S] order
+    for (int q = threadIdx.x; q < total; q += blockDim.x) rows[q] = ObsOut<T>::cv(0.0f);
+    __syncthreads();
+    if ((int)threadIdx.x < cnt) {
+        const int r = __ldg(slot_row + o + threadIdx.x);
+        hdr[o + threadIdx.x] = r >= 0 ? obs_observer<T>(P, a, r - __ldg(off + a), rows + (size_t)threadIdx.x * P.F)
+                                      : make_int4(0, 0, P.A, 0);
     }
+    __syncthreads();
+    obs_store_rows<T>((T *)P.feature + o * P.F, rows, total);
 }
 
 #ifndef OBS_WARPS_PER_SM
@@ -1742,24 +1785,35 @@ static void launch_obs_render(Ctx *c, const ObsArgs &O, ObsParams &P, int n_tota
     if (timed) CUDA_CHECK(cudaEventRecord(e1, c->stream));
 }
 
+// scratch owned by the context: the per-agent headers of n observers
+static void grow_obs_hdr(Ctx *c, size_t n) {
+    if (n <= c->obs_hdr_n) return;
+    no_capture(c, "growing the observation header table");
+    if (c->obs_hdr) { CUDA_CHECK(cudaStreamSynchronize(c->stream)); cudaFree(c->obs_hdr); }
+    c->obs_hdr_n = n + n / 4 + 64;
+    CUDA_CHECK(cudaMalloc(&c->obs_hdr, c->obs_hdr_n * sizeof(int4)));
+}
+
+// threads per CTA of the header pre-passes: as many observers as fit 48 KB of feature rows (*smem bytes)
+static int obs_prepass_threads(int F, size_t elem, size_t *smem) {
+    int threads = 256;
+    while (threads > 32 && (size_t)threads * F * elem > 48 * 1024) threads >>= 1;
+    *smem = (size_t)threads * F * elem;
+    if (*smem > 48 * 1024) mg::fatal("feature row too long for the header kernel (%d elements)", F);
+    return threads;
+}
+
 // cfg_slot: 0..5, one per (T, NIT, TURN); each owns two context slots, one per tile width
 template <typename T, int NIT, bool TURN>
 static void launch_obs_typed(Ctx *c, int cfg_slot, const EngineDev &hE, const ObsArgs &O, ObsParams &P, int n_total,
                              int view_count, bool with_headers = true, bool headers_only = false) {
     if (obs_all_cells_in_regs<NIT, TURN>() && view_count > NIT * 32)
         mg::fatal("render kernel NIT=%d chosen for a view of %d in-range cells", NIT, view_count);
-    if ((size_t)n_total > c->obs_hdr_n) {                                // scratch owned by the context: per-agent headers
-        no_capture(c, "growing the observation header table");
-        if (c->obs_hdr) { CUDA_CHECK(cudaStreamSynchronize(c->stream)); cudaFree(c->obs_hdr); }
-        c->obs_hdr_n = (size_t)n_total + n_total / 4 + 64;
-        CUDA_CHECK(cudaMalloc(&c->obs_hdr, c->obs_hdr_n * sizeof(int4)));
-    }
+    grow_obs_hdr(c, (size_t)n_total);
     P.hdr = c->obs_hdr;
     if (with_headers) {
-        int threads = 256;                                               // as many observers per CTA as fit 48 KB of rows
-        while (threads > 32 && (size_t)threads * P.F * sizeof(T) > 48 * 1024) threads >>= 1;
-        const size_t hsm = (size_t)threads * P.F * sizeof(T);
-        if (hsm > 48 * 1024) mg::fatal("feature row too long for the header kernel (%d elements)", P.F);
+        size_t hsm;
+        const int threads = obs_prepass_threads(P.F, sizeof(T), &hsm);
         const int cpa = (P.cap + threads - 1) / threads;
         obs_headers_kernel<T><<<(unsigned)((size_t)P.A * cpa), threads, hsm, c->stream>>>(P, c->obs_hdr, cpa);
         post_launch("obs_headers_kernel");
@@ -2448,6 +2502,67 @@ void dma_wait(Ctx *c, int keep_in_flight) {
         CUDA_CHECK(cudaEventSynchronize(c->dma_events[c->dma_head % c->dma_events.size()]));
         ++c->dma_head;
     }
+}
+
+// ------------------------------------------------------------------------------------------------
+// slot-ordered observations (magent_b200_get_observation_slots): record a * S + s is the record env_get_observation
+// writes for the row in slot s of arena a, all zeros where the slot is vacant.  Only the pre-pass knows about slots:
+// slots_kernel writes the [A][S] slot -> row map into scratch, obs_slot_headers_kernel one header and one feature row
+// per slot, and the unchanged obs_render_kernel renders the A * S headers as it renders rows.  A vacant slot's header
+// names the blank arena A at (0, 0), self cell 0:
+//   * its kind plane is the zeroed window the engine keeps after the last arena's plane in EngineDev::kind: (2 kpad + 1)
+//     rows of kw bytes, which hold every view cell of an observer at (0, 0).  No cell is marked, so the hp_norm plane is
+//     never read;
+//   * its minimap row is row A of mm_pad: zeros, but -1 at cell 0 of every group, so the self marker (+1 at cell 0)
+//     leaves +0 there and the undo between two vacant records puts the -1 back.
+// A vacant record next to a live one in a CTA's chunk is an arena change, so the render rebuilds the record.  The
+// render bounds its record count by the device-side total of the rows (P.off[P.A]); here every one of the A * S headers
+// is valid whatever the counts, so P.off points at [A + 1] words of INT_MAX.
+__global__ void __launch_bounds__(256) obs_blank_minimap_kernel(float *row, int G, int cells) {
+    for (int k = threadIdx.x; k < G * cells; k += blockDim.x) row[k] = k % cells == 0 ? -1.0f : 0.0f;
+}
+
+void launch_obs_slots(Ctx *c, const EngineDev *, const EngineDev &hE, const SlotDev *T, const ObsArgs &O,
+                      const float *mm_val, int S) {
+    DeviceGuard guard(c);
+    const size_t n = (size_t)hE.A * S;
+    if (n == 0) return;
+    if (n > 0x7fffffff) mg::fatal("%zu slot-ordered observation records are more than one launch renders", n);
+    grow_obs_hdr(c, n);
+    if (n > c->obs_slot_row_n) {
+        no_capture(c, "growing the slot table of the observation pre-pass");
+        grow_dev(c, c->obs_slot_row, c->obs_slot_row_n, n);
+    }
+    if ((size_t)hE.A + 1 > c->obs_slot_bound_n) {
+        no_capture(c, "growing the observation count bound");
+        if (c->obs_slot_bound) { CUDA_CHECK(cudaStreamSynchronize(c->stream)); cudaFree(c->obs_slot_bound); }
+        c->obs_slot_bound_n = (size_t)hE.A + 1;
+        CUDA_CHECK(cudaMalloc(&c->obs_slot_bound, c->obs_slot_bound_n * sizeof(int)));
+        const std::vector<int> bound(c->obs_slot_bound_n, 0x7fffffff);
+        CUDA_CHECK(cudaMemcpyAsync(c->obs_slot_bound, bound.data(), bound.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+        CUDA_CHECK(cudaStreamSynchronize(c->stream));
+    }
+    ObsParams P;
+    fill_obs_params(c, hE, O, mm_val, (int)n, P);
+    const int g = O.group;
+    const GroupDev &D = hE.grp[g];
+    const int *off = P.off;
+    slots_kernel<<<(unsigned)hE.A, SLOT_THREADS, 0, c->stream>>>(off, D.soa[(O.curmask >> g) & 1u].id, D.cap, T, hE.A, S,
+                                                                 nullptr, c->obs_slot_row, 0x7fffffff);
+    post_launch("slots_kernel");
+    if (mm_val) {
+        obs_blank_minimap_kernel<<<1, 256, 0, c->stream>>>(c->mm_pad + (size_t)hE.A * c->mm_stride, hE.G, P.cells);
+        post_launch("obs_blank_minimap_kernel");
+    }
+    size_t hsm;
+    const int threads = obs_prepass_threads(P.F, O.half ? 2 : 4, &hsm);
+    const int cps = (S + threads - 1) / threads;
+    const unsigned grid = (unsigned)((size_t)hE.A * cps);
+    if (O.half) obs_slot_headers_kernel<__half><<<grid, threads, hsm, c->stream>>>(P, off, c->obs_slot_row, S, c->obs_hdr, cps);
+    else obs_slot_headers_kernel<float><<<grid, threads, hsm, c->stream>>>(P, off, c->obs_slot_row, S, c->obs_hdr, cps);
+    post_launch("obs_slot_headers_kernel");
+    P.off = c->obs_slot_bound;
+    launch_obs_dispatch(c, hE, O, P, (int)n, false, false);
 }
 
 }  // namespace be

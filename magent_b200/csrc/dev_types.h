@@ -178,7 +178,9 @@ struct EngineDev {
     int *occ, *claim_head;                    // [A][H*W]
     // observation planes, padded by kpad cells on every side so that a view window never needs a bounds check:
     // cell (x, y) of arena a lives at a * kplane + (y + kpad) * kw + x + kpad
-    unsigned char *kind;                      // [A][kplane] 0 empty / 1 wall / 2 + group; kept in step with occ
+    unsigned char *kind;                      // [A][kplane] 0 empty / 1 wall / 2 + group; kept in step with occ; then a
+                                              // window of (2 kpad + 1) * kw zero bytes: the blank arena A of vacant slots
+                                              // (backend_cuda.cu launch_obs_slots), whose observer stands at (0, 0)
     float *hpn;                               // [A][kplane] hp / max_hp of the occupant where kind lacks KIND_FULL; kept in step with hp
     int kpad, kw;
     long kplane;

@@ -847,7 +847,9 @@ void Engine::to_device() {
         hE_.food = food_mode_ ? (float *)dalloc(cells * 4) : nullptr;
         {   // padded observation planes (dev_types.h)
             hE_.kpad = pad; hE_.kw = W_ + 2 * pad; hE_.kplane = (long)hE_.kw * (H_ + 2 * pad);
-            hE_.kind = (unsigned char *)dalloc((size_t)A_ * hE_.kplane + 16);
+            const size_t blank = (size_t)(2 * pad + 1) * hE_.kw;          // the blank arena's window, zero for good
+            hE_.kind = (unsigned char *)dalloc((size_t)A_ * hE_.kplane + blank + 16);
+            be::dmemset(bx_, hE_.kind + (size_t)A_ * hE_.kplane, 0, blank + 16);
             hE_.hpn = (float *)dalloc(((size_t)A_ * hE_.kplane + 4) * 4);
             be::dmemset(bx_, hE_.hpn, 0, ((size_t)A_ * hE_.kplane + 4) * 4);
         }
@@ -1073,6 +1075,18 @@ void Engine::stage_reserve(void *&p, size_t &have, size_t need) {
     p = be::dmalloc(bx_, have);
 }
 
+// The observation pre-pass (normalised minimap) for group's observers, unless the last one still holds: its products
+// depend on the state, on the observer's view size (minimap grid) and on whether the observer's type skips absorbed
+// agents in the minimap (GridWorld.cc:343-347)
+void Engine::prepare_obs(int group) {
+    const AgentTypeDef &t = *group_type_[group];
+    if (prep_version_ != state_version_ || prep_vw_ != t.view.width || prep_vh_ != t.view.height ||
+        prep_skip_absorbed_ != t.can_absorb) {
+        be::launch_obs_prepare(bx_, dE_, hE_, curmask_, group, minimap_mode_ ? d_mm_val_ : nullptr);
+        prep_version_ = state_version_; prep_vw_ = t.view.width; prep_vh_ = t.view.height; prep_skip_absorbed_ = t.can_absorb;
+    }
+}
+
 void Engine::get_observation(int group, void **bufs, int half) {      // GridWorld.cc:292-401
     check_group(group, "GridWorld::get_observation");
     to_device();
@@ -1084,13 +1098,7 @@ void Engine::get_observation(int group, void **bufs, int half) {      // GridWor
     const size_t vbytes = (size_t)n * t.view.height * t.view.width * n_channel() * esz;
     const size_t fbytes = (size_t)n * feature_size(group) * esz;
     const bool vdev = be::is_device_ptr(bufs[0]), fdev = be::is_device_ptr(bufs[1]);
-    // the pre-pass products depend on the state, on the observer's view size (minimap grid) and on whether the
-    // observer's type skips absorbed agents in the minimap (GridWorld.cc:343-347)
-    if (prep_version_ != state_version_ || prep_vw_ != t.view.width || prep_vh_ != t.view.height ||
-        prep_skip_absorbed_ != t.can_absorb) {
-        be::launch_obs_prepare(bx_, dE_, hE_, curmask_, group, minimap_mode_ ? d_mm_val_ : nullptr);
-        prep_version_ = state_version_; prep_vw_ = t.view.width; prep_vh_ = t.view.height; prep_skip_absorbed_ = t.can_absorb;
-    }
+    prepare_obs(group);
     if (host_path_ < 0) {                 // MAGENT_B200_HOST_PATH=dense keeps the round-1 path (dense records over PCIe) for A/B runs
         const char *e = getenv("MAGENT_B200_HOST_PATH");                 // dense | wire (whatever the size) | default: by size
         host_path_ = (e && !strcmp(e, "dense")) ? 0 : (e && !strcmp(e, "wire")) ? 2 : 1;
@@ -1461,6 +1469,41 @@ int Engine::get_slots(int group, int *row_slot, int *slot_row) {
     read_back(mem == 1, {{row_slot, (size_t)nb * 4}, {slot_row, (size_t)A_ * S * 4}}, [&](void **to) {
         be::launch_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, (int *)to[0], (int *)to[1], nb);
     });
+    return 0;
+}
+
+// The observation of one group in slot order, [A][S] records and feature rows.  Its shape needs no counts (the device
+// decides which slots hold rows), so neither pointer kind waits for them.  Device buffers: no staging, allocation or
+// synchronisation once warm.  Host buffers: through the device staging of the dense observations, copied back.
+int Engine::get_observation_slots(int group, void **bufs, int half) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_observation_slots", group);
+    if (half != 0 && half != 1) return refuse("get_observation_slots: half must be 0 or 1, not %d", half);
+    if (!bufs || !bufs[0] || !bufs[1]) return refuse("get_observation_slots needs a view and a feature buffer");
+    if (!be::launch_obs_slots || !be::launch_restore_slots)
+        return refuse("the %s backend has no slot-ordered observation kernel", be::name());
+    const int mem = out_memory("get_observation_slots: view and feature", {bufs[0], bufs[1]});
+    if (mem < 0) return -1;
+    to_device();
+    const int S = group < (int)slot_space_.size() ? slot_space_[group] : 0;
+    if (S == 0) return 0;
+    const AgentTypeDef &t = *group_type_[group];
+    const size_t esz = half ? 2 : 4, n = (size_t)A_ * S;
+    const size_t vbytes = n * t.view.height * t.view.width * n_channel() * esz, fbytes = n * feature_size(group) * esz;
+    prepare_obs(group);
+    ObsArgs O;
+    O.curmask = curmask_; O.group = group; O.half = half;
+    O.grid = obs_grid_; O.chunk = obs_chunk_; O.tile = obs_tile_;
+    if (mem == 1) {
+        O.view = bufs[0]; O.feature = bufs[1];
+    } else {
+        stage_reserve(d_view_stage_, view_stage_bytes_, vbytes); O.view = d_view_stage_;
+        stage_reserve(d_feat_stage_, feat_stage_bytes_, fbytes); O.feature = d_feat_stage_;
+    }
+    be::launch_obs_slots(bx_, dE_, hE_, d_slot_dev_, O, minimap_mode_ ? d_mm_val_ : nullptr, S);
+    if (mem == 0) {
+        be::d2h(bx_, bufs[0], d_view_stage_, vbytes); io_[IO_D2H] += (long long)vbytes;
+        be::d2h(bx_, bufs[1], d_feat_stage_, fbytes); io_[IO_D2H] += (long long)fbytes;
+    }
     return 0;
 }
 

@@ -141,6 +141,10 @@ public:
     // stable slots (slot_phases.h): int [num_bound] row -> a * S + slot and int [A][S] slot -> row of one group, S =
     // slot_space(group); either may be null, not both.  -1 and the last error when refused.
     int get_slots(int group, int *row_slot, int *slot_row);
+    // the observation of one group in slot order: bufs[0] view [A][S][view_h][view_w][n_channel], bufs[1] feature
+    // [A][S][feature_size], the records get_observation writes for the row in each slot, all zeros in vacant slots;
+    // half: IEEE binary16.  -1 and the last error when refused.
+    int get_observation_slots(int group, void **bufs, int half);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads
@@ -262,6 +266,7 @@ private:
     struct OutPart { void *buf; size_t bytes; };
     template <size_t N, class F> void read_back(bool dev, const OutPart (&parts)[N], F &&launch);
     void stage_reserve(void *&p, size_t &have, size_t need);
+    void prepare_obs(int group);        // the observation pre-pass for group's observers, unless still valid
     void get_observation_wire(int group, void **bufs);
     int max_agents_per_arena() const;
 

@@ -117,6 +117,9 @@ MG_API int magent_b200_get_neighbours(EnvHandle game, GroupHandle group, GroupHa
 MG_API int magent_b200_get_slots(EnvHandle game, GroupHandle group, int *row_slot, int *slot_row) {
     return E(game)->get_slots(group, row_slot, slot_row);
 }
+MG_API int magent_b200_get_observation_slots(EnvHandle game, GroupHandle group, void **buffer, int half) {
+    return E(game)->get_observation_slots(group, buffer, half);
+}
 MG_API int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **buffer) {
     E(game)->get_observation(group, buffer, 1);
     return 0;

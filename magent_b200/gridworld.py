@@ -759,6 +759,51 @@ class GridWorld(Environment):
         self._check(self._lib.magent_b200_get_slots(self.game, g, _dptr(row_slot), _dptr(slot_row)), "get_slots")
         return row_slot, slot_row
 
+    def get_observation_slots(self, handle):
+        """(views, features) of a whole group in the stable slot layout (see get_slots): float32
+        (num_arenas, S) + view_space and (num_arenas, S) + feature_space, S = get_slot_space(handle).  Slot (a, s) holds
+        the record get_observation gives the row slot_row[a, s]; a vacant slot is all zeros.  The arrays are cached
+        receive buffers: valid until the next call."""
+        g = self._hv(handle)
+        lead = (self.num_arenas, self.get_slot_space(handle))
+        view = self._host_view((g, "view_slots"), lead + self.view_space[g], np.float32)
+        feat = self._host_view((g, "feature_slots"), lead + self.feature_space[g], np.float32)
+        if view.size:
+            bufs = (ctypes.c_void_p * 2)(view.ctypes.data, feat.ctypes.data)
+            self._check(self._lib.magent_b200_get_observation_slots(self.game, g, bufs, 0), "get_observation_slots")
+        return view, feat
+
+    def get_observation_slots_torch(self, handle, out=None, dtype=None):
+        """the slot-ordered observation (see get_observation_slots) rendered straight into CUDA tensors, without waiting
+        for the device: (view (num_arenas, S) + view_space, feature (num_arenas, S) + feature_space).
+
+        dtype: torch.float32 (default) or torch.float16 (every element the float32 value rounded to nearest-even).
+        out: a caller-owned (view, feature) pair of contiguous CUDA tensors of those shapes and one dtype; needed to
+        record the call into a CUDA graph (capture_graph), since the call then allocates nothing once a first call has
+        run."""
+        import torch
+        g = self._hv(handle)
+        lead = (self.num_arenas, self.get_slot_space(handle))
+        shapes = (lead + self.view_space[g], lead + self.feature_space[g])
+        if out is None:
+            dtype = torch.float32 if dtype is None else dtype
+            if dtype not in (torch.float32, torch.float16):
+                raise ValueError("observation dtype must be torch.float32 or torch.float16")
+            view, feat = (torch.empty(s, dtype=dtype, device="cuda") for s in shapes)
+        else:
+            if not isinstance(out, (tuple, list)) or len(out) != 2:
+                raise ValueError("out must be a (view, feature) pair of CUDA tensors")
+            view, feat = out
+            dtypes = (torch.float32, torch.float16) if dtype is None else (dtype,)
+            _check_cuda_out(view, "view", dtypes, shape=shapes[0])
+            _check_cuda_out(feat, "feature", (view.dtype,), shape=shapes[1])
+        if view.numel():
+            bufs = (ctypes.c_void_p * 2)(view.data_ptr(), feat.data_ptr())
+            self._check(self._lib.magent_b200_get_observation_slots(self.game, g, bufs,
+                                                                    1 if view.dtype == torch.float16 else 0),
+                        "get_observation_slots")
+        return view, feat
+
     def get_counters(self):
         """int64 event counters accumulated on the device since construction"""
         buf = (ctypes.c_longlong * 16)()
