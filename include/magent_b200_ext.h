@@ -127,6 +127,39 @@ int magent_b200_get_slots(EnvHandle game, GroupHandle group, int *row_slot, int 
  * magent_b200_last_error and writes nothing for a bad group handle, half other than 0 or 1, a NULL pointer, pointers that
  * mix host and CUDA device memory, or a backend without the kernel. */
 int magent_b200_get_observation_slots(EnvHandle game, GroupHandle group, void **buffer, int half);
+/* The rest of a fixed-shape step loop in the [arena, slot] layout of magent_b200_get_slots: actions in, rewards, agent
+ * status and legal-action masks out.  S = env_get_info(game, -1, "slot_space", int[n_group])[group], A = num_arenas.
+ * The shapes are known on the host and the device decides which slots hold rows (the device-side offsets and the slot
+ * table), so none of the three calls waits for the agent counts, whatever the pointer kind.  Both CUDA device pointers:
+ * no synchronisation and no allocation (get_action_mask_slots: once a first call has sized the engine's tables), so
+ * the calls can be recorded into a CUDA graph, also after a restore from a device src inside the graph.  They cover
+ * every arena whatever magent_b200_select_arena says.
+ *
+ * set_action_slots: act is int32 [A][S].  Every agent of the group, at its row r below the device-side count, takes
+ * act[a * S + slot] as its action, (a, slot) being its arena and slot.  Values in vacant slots are never read, so they
+ * may be anything, out-of-range ids included.  The engine state afterwards is bit for bit what env_set_action(game, group,
+ * rows) leaves with rows[r] = act[row_slot[r]], including every later step output and magent_b200_get_mean_action.  The
+ * call is the group's set_action for this step: it takes the same place in the step's action order, makes
+ * magent_b200_restore_arenas refuse until env_step as set_action does, and a second call for the group in the same step
+ * (this one or env_set_action) overwrites.  S == 0: only registers the group's action, reads nothing, act may be NULL.
+ * A host act is copied in (A * S * 4 bytes, counted in the h2d figure of magent_b200_get_io_stats).  Returns -1, sets
+ * magent_b200_last_error, writes nothing and registers nothing for a bad group handle, a NULL act when S > 0, or a
+ * backend without the kernel. */
+int magent_b200_set_action_slots(EnvHandle game, GroupHandle group, const int *act);
+/* reward[a][s] = bit for bit the value env_get_reward gives the row in slot (a, s), +0.0 in a vacant slot
+ *                                                                                 float32 [A][S], may be NULL
+ * status[a][s] = 0 vacant, 1 the row's env_get_info("alive") is 1, 2 occupied by a dead agent that has not been culled
+ *                yet: between env_step and gridworld_clear_dead, 2 is the per-agent terminal signal; after the cull
+ *                those slots read 0                                               uint8 [A][S], may be NULL
+ * Either pointer may be NULL, but not both.  Host pointers are copied back and counted in the d2h figure, exactly the
+ * bytes asked for.  Returns -1, sets magent_b200_last_error and writes nothing for a bad group handle, two NULL pointers,
+ * pointers that mix host and CUDA device memory, or a backend without the kernel. */
+int magent_b200_get_reward_slots(EnvHandle game, GroupHandle group, float *reward, unsigned char *status);
+/* mask uint8 [A][S][n_action]: an occupied slot's row is bit for bit the row magent_b200_get_action_mask gives its
+ * agent's row (a dead, un-culled agent's row is all zero); a vacant slot's row is all zero.  Host pointer: copied back
+ * and counted in the d2h figure.  Returns -1, sets magent_b200_last_error and writes nothing for a bad group handle, a
+ * NULL mask, or a backend without the kernel. */
+int magent_b200_get_action_mask_slots(EnvHandle game, GroupHandle group, unsigned char *mask);
 /* compact observation hand-off (SURVEY.md 8f rank 2): same call, layout and pointer rules as env_get_observation
  * (reference src/runtime_api.h:35), but every element is an IEEE binary16 = the float32 value rounded to
  * nearest-even.  buffer[0] = view [n][view_h][view_w][n_channel], buffer[1] = feature [n][feature_size];

@@ -111,6 +111,18 @@ __attribute__((weak)) void launch_restore_slots(Ctx *, const EngineDev *dE, cons
 // EngineDev::kind.  Weak like launch_slots: the engine refuses the call without it.
 __attribute__((weak)) void launch_obs_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
                                             const ObsArgs &O, const float *mm_val, int S);
+// The slot-ordered step loop of `group` (slot_phases.h, the device-side offsets decide the rows; all buffers are device
+// buffers of [A][S] entries).  launch_set_action_slots: every row's AgentSoA::act = act[its slot], nothing else is read.
+// launch_reward_slots: reward[slot] = the row's env_get_reward value and status[slot] = 1 alive, 2 dead (not culled yet),
+// +0.0 and 0 where no row is; either may be null.  launch_action_mask_slots: mask [A][S][n_action], the row
+// launch_action_mask writes for the row in each slot (mask_phases.h action_legal), all zero where no row is.  Weak like
+// launch_slots: the engine refuses the calls without them.
+__attribute__((weak)) void launch_set_action_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
+                                                   unsigned curmask, int group, int S, const int *act);
+__attribute__((weak)) void launch_reward_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
+                                               unsigned curmask, int group, int S, float *reward, unsigned char *status);
+__attribute__((weak)) void launch_action_mask_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
+                                                    unsigned curmask, int group, int S, unsigned char *mask);
 // clear_dead: asynchronous read-back of the [G][A+1] offset table (launch_offsets) into page-locked memory
 void counts_fetch_begin(Ctx *, const int *dev_off, size_t n_ints);
 const int *counts_fetch_wait(Ctx *);     // blocks until the fetch has landed; valid until the next counts_fetch_begin

@@ -75,8 +75,8 @@ struct Ctx {
     float *mm_pad = nullptr; size_t mm_pad_n = 0; int mm_stride = 0;
     // per-observer headers of the render kernel
     int4 *obs_hdr = nullptr; size_t obs_hdr_n = 0;
-    // slot-ordered observations (launch_obs_slots): the [A][S] slot -> row scratch, and the render's count bound
-    // ([A + 1] words of INT_MAX)
+    // slot-ordered observations (launch_obs_slots): the [A][S] slot -> row scratch (launch_action_mask_slots uses it
+    // too), and the render's count bound ([A + 1] words of INT_MAX)
     int *obs_slot_row = nullptr; size_t obs_slot_row_n = 0;
     int *obs_slot_bound = nullptr; size_t obs_slot_bound_n = 0;
     // cudaFuncSetAttribute caches (per device: a context never changes device)
@@ -770,6 +770,17 @@ __device__ __forceinline__ int mask_warp_setup(const EngineDev &E, unsigned curm
     return cta_cnt;
 }
 
+// The `total` bytes a CTA composed at `rows` (mask_smem + the 16-byte phase of `dst`) into `dst`: a byte head up to the
+// first 16-byte boundary, 16 bytes per thread in the body, a byte tail.  Every thread of the CTA calls it after a barrier.
+__device__ __forceinline__ void mask_rows_store(unsigned char *dst, const unsigned char *rows, int total) {
+    const int shift = (int)((size_t)dst & 15);
+    const int head = min(total, (16 - shift) & 15);
+    const int body = (total - head) >> 4;
+    for (int q = threadIdx.x; q < head; q += MASK_THREADS) dst[q] = rows[q];
+    for (int q = threadIdx.x; q < body; q += MASK_THREADS) ((uint4 *)(dst + head))[q] = ((const uint4 *)(rows + head))[q];
+    for (int q = head + (body << 4) + threadIdx.x; q < total; q += MASK_THREADS) dst[q] = rows[q];
+}
+
 __global__ void __launch_bounds__(MASK_THREADS) action_mask_kernel(const EngineDev *gE, unsigned curmask, int g,
                                                                   unsigned char *out, int n_total, int chunks_per_arena) {
     __shared__ EngineDev sE;
@@ -792,12 +803,7 @@ __global__ void __launch_bounds__(MASK_THREADS) action_mask_kernel(const EngineD
         for (int k = lane; k < na; k += 32) row[k] = action_legal(E, curmask, w.a, occ, g, m, k) ? 1 : 0;
     }
     __syncthreads();
-    const int total = cta_cnt * na;
-    const int head = min(total, (16 - shift) & 15);
-    const int body = (total - head) >> 4;
-    for (int q = threadIdx.x; q < head; q += MASK_THREADS) dst[q] = rows[q];
-    for (int q = threadIdx.x; q < body; q += MASK_THREADS) ((uint4 *)(dst + head))[q] = ((const uint4 *)(rows + head))[q];
-    for (int q = head + (body << 4) + threadIdx.x; q < total; q += MASK_THREADS) dst[q] = rows[q];
+    mask_rows_store(dst, rows, cta_cnt * na);
 }
 
 // The byte mask is never materialised: one thread per agent counts its legal actions, draws r = legal_draw(...) below
@@ -2563,6 +2569,127 @@ void launch_obs_slots(Ctx *c, const EngineDev *, const EngineDev &hE, const Slot
     post_launch("obs_slot_headers_kernel");
     P.off = c->obs_slot_bound;
     launch_obs_dispatch(c, hE, O, P, (int)n, false, false);
+}
+
+// ------------------------------------------------------------------------------------------------
+// the slot-ordered step loop (magent_b200_set_action_slots, _get_reward_slots, _get_action_mask_slots), slot_phases.h.
+// Actions: one thread per row, CTAs dealt per arena like info_kernel; each row looks its agent's id up in the slot table
+// and loads its action from the [A][S] buffer.  Reward and status: one CTA per arena like slots_kernel, which fills the
+// arena's [S] blocks, then scatters its rows; no scratch, so the call records into a graph from its first use.
+__global__ void __launch_bounds__(256) set_action_slots_kernel(const EngineDev *gE, unsigned curmask, int g,
+                                                               const SlotDev *T, int S, const int *act,
+                                                               int chunks_per_arena) {
+    const EngineDev &E = *gE;
+    const int *off = E.off + (size_t)g * (E.A + 1);
+    const AgentSoA &s = E.grp[g].soa[(curmask >> g) & 1u];
+    const int a = blockIdx.x / chunks_per_arena;
+    const int i = (blockIdx.x - a * chunks_per_arena) * blockDim.x + threadIdx.x;
+    if (i >= off[a + 1] - off[a]) return;
+    const long gi = (long)a * E.grp[g].cap + i;
+    const int flat = slot_flat(T->tab, T->id_cap, a, s.id[gi], S);
+    if (flat >= 0) s.act[gi] = __ldg(act + flat);
+}
+
+void launch_set_action_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, const SlotDev *T, unsigned curmask,
+                             int group, int S, const int *act) {
+    DeviceGuard guard(c);
+    const int cap = hE.grp[group].cap;
+    const int threads = cap >= 256 ? 256 : ((cap + 31) & ~31);
+    const int cpa = (cap + threads - 1) / threads;
+    set_action_slots_kernel<<<(unsigned)((size_t)hE.A * cpa), threads, 0, c->stream>>>(dE, curmask, group, T, S, act, cpa);
+    post_launch("set_action_slots_kernel");
+}
+
+__global__ void __launch_bounds__(SLOT_THREADS) reward_slots_kernel(const EngineDev *gE, unsigned curmask, int g,
+                                                                    const SlotDev *T, int S, float *reward,
+                                                                    unsigned char *status) {
+    const EngineDev &E = *gE;
+    const int a = blockIdx.x;
+    for (int q = threadIdx.x; q < S; q += SLOT_THREADS) {
+        if (reward) reward[(long)a * S + q] = 0.0f;
+        if (status) status[(long)a * S + q] = 0;
+    }
+    __syncthreads();
+    const int *off = E.off + (size_t)g * (E.A + 1);
+    const AgentSoA &s = E.grp[g].soa[(curmask >> g) & 1u];
+    const int o0 = off[a], cnt = off[a + 1] - o0;
+    const float shared_reward = E.hdr[a].grp_reward[g];
+    const long base = (long)a * E.grp[g].cap;
+    for (int i = threadIdx.x; i < cnt; i += SLOT_THREADS) {
+        const int flat = slot_flat(T->tab, T->id_cap, a, s.id[base + i], S);
+        if (flat < 0) continue;
+        if (reward) reward[flat] = s.next_reward[base + i] + shared_reward;        // info_kernel's INFO_REWARD
+        if (status) status[flat] = (s.flags[base + i] & FLAG_DEAD) ? 2 : 1;
+    }
+}
+
+void launch_reward_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, const SlotDev *T, unsigned curmask, int group,
+                         int S, float *reward, unsigned char *status) {
+    DeviceGuard guard(c);
+    reward_slots_kernel<<<(unsigned)hE.A, SLOT_THREADS, 0, c->stream>>>(dE, curmask, group, T, S, reward, status);
+    post_launch("reward_slots_kernel");
+}
+
+// Mask: slots_kernel writes the [A][S] slot -> row map into the scratch of the slot-ordered observation, then
+// action_mask_slots_kernel takes MASK_THREADS consecutive slots of one arena per CTA, so an arena gets several CTAs
+// whatever its population (a one-arena batch is not one CTA).  It is action_mask_kernel with the lanes' agents looked up
+// through the map: a vacant slot's lane holds a dead agent, which action_legal refuses every action, so its row is zero.
+// The CTA's rows are one contiguous byte range of the output, stored as action_mask_kernel stores its rows.
+__global__ void __launch_bounds__(MASK_THREADS) action_mask_slots_kernel(const EngineDev *gE, unsigned curmask, int g,
+                                                                        const int *slot_row, int S, unsigned char *out,
+                                                                        int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    extern __shared__ __align__(16) unsigned char mask_smem[];
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int a = blockIdx.x / chunks_per_arena;
+    const int c0 = (blockIdx.x - a * chunks_per_arena) * MASK_THREADS;
+    const int cta_cnt = min(MASK_THREADS, S - c0);
+    const int cnt = min(32, cta_cnt - 32 * warp);
+    MaskAgent mine;
+    mine.x = mine.y = 0; mine.dir = DIR_NORTH; mine.code = 0; mine.flags = FLAG_DEAD;
+    if (lane < cnt) {
+        const int r = slot_row[(long)a * S + c0 + 32 * warp + lane];
+        if (r >= 0) mine = mask_agent(E, curmask, a, g, r - E.off[(size_t)g * (E.A + 1) + a]);
+    }
+    const int na = E.grp[g].n_action;
+    unsigned char *dst = out + ((size_t)a * S + c0) * na;
+    unsigned char *rows = mask_smem + ((size_t)dst & 15);
+    const int *occ = E.occ + (long)a * E.W * E.H;
+    for (int j = 0; j < cnt; ++j) {
+        MaskAgent m;
+        m.x = __shfl_sync(0xffffffffu, mine.x, j); m.y = __shfl_sync(0xffffffffu, mine.y, j);
+        m.dir = __shfl_sync(0xffffffffu, mine.dir, j); m.code = __shfl_sync(0xffffffffu, mine.code, j);
+        m.flags = (unsigned char)__shfl_sync(0xffffffffu, (int)mine.flags, j);
+        unsigned char *row = rows + (size_t)(32 * warp + j) * na;
+        for (int k = lane; k < na; k += 32) row[k] = action_legal(E, curmask, a, occ, g, m, k) ? 1 : 0;
+    }
+    __syncthreads();
+    mask_rows_store(dst, rows, cta_cnt * na);
+}
+
+void launch_action_mask_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, const SlotDev *T, unsigned curmask,
+                              int group, int S, unsigned char *mask) {
+    DeviceGuard guard(c);
+    const size_t n = (size_t)hE.A * S;
+    if (n == 0) return;
+    const int na = hE.grp[group].n_action;
+    const size_t smem = (size_t)MASK_THREADS * na + 16;
+    if (smem + sizeof(EngineDev) > 48 * 1024) mg::fatal("action mask: %d actions per agent are more than the kernels hold", na);
+    if (n > c->obs_slot_row_n) {
+        no_capture(c, "growing the slot table of the slot-ordered action mask");
+        grow_dev(c, c->obs_slot_row, c->obs_slot_row_n, n);
+    }
+    const GroupDev &D = hE.grp[group];
+    slots_kernel<<<(unsigned)hE.A, SLOT_THREADS, 0, c->stream>>>(hE.off + (size_t)group * (hE.A + 1),
+                                                                 D.soa[(curmask >> group) & 1u].id, D.cap, T, hE.A, S,
+                                                                 nullptr, c->obs_slot_row, 0x7fffffff);
+    post_launch("slots_kernel");
+    const int cps = (S + MASK_THREADS - 1) / MASK_THREADS;
+    action_mask_slots_kernel<<<(unsigned)((size_t)hE.A * cps), MASK_THREADS, smem, c->stream>>>(dE, curmask, group,
+                                                                                               c->obs_slot_row, S, mask, cps);
+    post_launch("action_mask_slots_kernel");
 }
 
 }  // namespace be

@@ -1507,6 +1507,64 @@ int Engine::get_observation_slots(int group, void **bufs, int half) {
     return 0;
 }
 
+// The slot-ordered step loop.  [A][S] is known on the host and the device decides which slots hold rows, so none of the
+// three calls waits for the counts; with CUDA pointers they neither synchronise nor allocate (the mask once warm).
+
+// set_action in slot order: every row below the device-side count takes act[its slot].  It is the group's set_action
+// for this step, registered in order_ as set_action registers it, once nothing can refuse the call any more.
+int Engine::set_action_slots(int group, const int *act) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in set_action_slots", group);
+    if (!be::launch_set_action_slots || !be::launch_restore_slots)
+        return refuse("the %s backend has no slot-ordered action kernel", be::name());
+    const int S = slot_space(group);
+    if (S > 0 && !act) return refuse("set_action_slots needs an action buffer");
+    to_device();
+    if (std::find(order_.begin(), order_.end(), group) == order_.end()) order_.push_back(group);
+    if (S == 0) return 0;
+    const void *src = act;
+    if (!be::is_device_ptr(act)) {
+        const size_t bytes = (size_t)A_ * S * 4;
+        void *st = io_stage(bytes);
+        be::h2d(bx_, st, act, bytes);
+        io_[IO_H2D] += (long long)bytes;
+        src = st;
+    }
+    be::launch_set_action_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, (const int *)src);
+    return 0;
+}
+
+// env_get_reward and the alive flag in slot order: float [A][S] and uint8 [A][S] (0 vacant, 1 alive, 2 dead)
+int Engine::get_reward_slots(int group, float *reward, unsigned char *status) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_reward_slots", group);
+    if (!reward && !status) return refuse("get_reward_slots needs a reward or a status buffer");
+    if (!be::launch_reward_slots || !be::launch_restore_slots)
+        return refuse("the %s backend has no slot-ordered reward kernel", be::name());
+    const int mem = out_memory("get_reward_slots: reward and status", {reward, status});
+    if (mem < 0) return -1;
+    to_device();
+    const int S = slot_space(group);
+    const size_t n = (size_t)A_ * S;
+    read_back(mem == 1, {{reward, n * 4}, {status, n}}, [&](void **to) {
+        be::launch_reward_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, (float *)to[0], (unsigned char *)to[1]);
+    });
+    return 0;
+}
+
+// The legal-action mask in slot order: uint8 [A][S][n_action]
+int Engine::get_action_mask_slots(int group, unsigned char *mask) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_action_mask_slots", group);
+    if (!mask) return refuse("get_action_mask_slots needs a mask buffer");
+    if (!be::launch_action_mask_slots || !be::launch_restore_slots)
+        return refuse("the %s backend has no slot-ordered action-mask kernel", be::name());
+    const int mem = out_memory("get_action_mask_slots: mask", {mask});
+    to_device();
+    const int S = slot_space(group);
+    read_back(mem == 1, {{mask, (size_t)A_ * S * group_type_[group]->n_action}}, [&](void **to) {
+        be::launch_action_mask_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, (unsigned char *)to[0]);
+    });
+    return 0;
+}
+
 void Engine::step(int *done) {                                        // GridWorld.cc:456-631
     to_device();
     StepArgs S;

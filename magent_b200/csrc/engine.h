@@ -145,6 +145,14 @@ public:
     // [A][S][feature_size], the records get_observation writes for the row in each slot, all zeros in vacant slots;
     // half: IEEE binary16.  -1 and the last error when refused.
     int get_observation_slots(int group, void **bufs, int half);
+    // the slot-ordered step loop (S = slot_space(group), [A][S] buffers; neither waits for the counts).  set_action_slots:
+    // set_action with act[slot] for every row, registered in the step's action order like set_action (act may be null
+    // when S == 0).  get_reward_slots: float reward and uint8 status (0 vacant, 1 alive, 2 dead, not culled yet) per
+    // slot, either may be null, not both.  get_action_mask_slots: uint8 [A][S][n_action], get_action_mask's row for the
+    // row in each slot, zero in vacant slots.  -1 and the last error when refused.
+    int set_action_slots(int group, const int *act);
+    int get_reward_slots(int group, float *reward, unsigned char *status);
+    int get_action_mask_slots(int group, unsigned char *mask);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads
@@ -218,6 +226,7 @@ private:
     std::vector<int> slot_space_;
     void upload_slots();
     void update_slot_space();
+    int slot_space(int group) const { return group < (int)slot_space_.size() ? slot_space_[group] : 0; }
     size_t view_stage_bytes_ = 0, feat_stage_bytes_ = 0;
     void *d_io_stage_ = nullptr; size_t io_stage_bytes_ = 0;
     void *h_feat_stage_ = nullptr; size_t h_feat_stage_bytes_ = 0;      // page-locked staging of the feature rows (host path)

@@ -120,6 +120,15 @@ MG_API int magent_b200_get_slots(EnvHandle game, GroupHandle group, int *row_slo
 MG_API int magent_b200_get_observation_slots(EnvHandle game, GroupHandle group, void **buffer, int half) {
     return E(game)->get_observation_slots(group, buffer, half);
 }
+MG_API int magent_b200_set_action_slots(EnvHandle game, GroupHandle group, const int *act) {
+    return E(game)->set_action_slots(group, act);
+}
+MG_API int magent_b200_get_reward_slots(EnvHandle game, GroupHandle group, float *reward, unsigned char *status) {
+    return E(game)->get_reward_slots(group, reward, status);
+}
+MG_API int magent_b200_get_action_mask_slots(EnvHandle game, GroupHandle group, unsigned char *mask) {
+    return E(game)->get_action_mask_slots(group, mask);
+}
 MG_API int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **buffer) {
     E(game)->get_observation(group, buffer, 1);
     return 0;

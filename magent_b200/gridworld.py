@@ -804,6 +804,94 @@ class GridWorld(Environment):
                         "get_observation_slots")
         return view, feat
 
+    def _slot_shape(self, handle):
+        return (self.num_arenas, self.get_slot_space(handle))
+
+    def set_action_slots(self, handle, actions):
+        """set_action in the stable slot layout (see get_slots): every agent takes actions[a, s] of its arena and slot;
+        vacant slots are never read.  actions: an int32 numpy array (num_arenas, S) or a contiguous CUDA int32 tensor of
+        that shape (nothing waits for the device, and the call can be recorded into a CUDA graph).  It counts as the
+        group's set_action for the step (include/magent_b200_ext.h magent_b200_set_action_slots has the definition)."""
+        g = self._hv(handle)
+        shape = self._slot_shape(handle)
+        if isinstance(actions, np.ndarray):
+            if actions.dtype != np.int32 or actions.shape != shape:
+                raise ValueError("actions must be an int32 array of shape %s" % (shape,))
+            actions = np.ascontiguousarray(actions)
+            ptr = actions.ctypes.data if actions.size else None
+        else:
+            import torch
+            _check_cuda_out(actions, "actions (when not an int32 numpy array)", (torch.int32,), shape=shape)
+            ptr = _dptr(actions)
+        self._check(self._lib.magent_b200_set_action_slots(self.game, g, ptr), "set_action_slots")
+
+    def get_reward_slots(self, handle):
+        """(reward float32 (num_arenas, S), status uint8 (num_arenas, S)) in the stable slot layout: the reward get_reward
+        gives the agent in each slot and 0 vacant / 1 alive / 2 dead but not culled yet (between step and clear_dead, 2
+        is the per-agent terminal signal); +0.0 and 0 in vacant slots.  Both arrays are cached receive buffers: valid
+        until the next call."""
+        g = self._hv(handle)
+        shape = self._slot_shape(handle)
+        reward = self._host_view((g, "reward_slots"), shape, np.float32)
+        status = self._host_view((g, "status_slots"), shape, np.uint8)
+        if reward.size:
+            self._check(self._lib.magent_b200_get_reward_slots(self.game, g, reward.ctypes.data, status.ctypes.data),
+                        "get_reward_slots")
+        return reward, status
+
+    def get_reward_slots_torch(self, handle, out=None):
+        """the slot-ordered reward and status (see get_reward_slots) written straight into CUDA tensors, without waiting
+        for the device: (reward float32 (num_arenas, S), status uint8 (num_arenas, S)).
+
+        out: a caller-owned pair (reward, status) of contiguous CUDA tensors of those shapes and dtypes; needed to record
+        the call into a CUDA graph (capture_graph), since the call then allocates nothing.  Either may be None: it is
+        then not written, and None comes back in its place."""
+        import torch
+        g = self._hv(handle)
+        shape = self._slot_shape(handle)
+        if out is None:
+            reward = torch.empty(shape, dtype=torch.float32, device="cuda")
+            status = torch.empty(shape, dtype=torch.uint8, device="cuda")
+        else:
+            if not isinstance(out, (tuple, list)) or len(out) != 2 or (out[0] is None and out[1] is None):
+                raise ValueError("out must be a (reward, status) pair of CUDA tensors, at most one of them None")
+            reward, status = out
+            _check_cuda_out(reward, "reward", (torch.float32,), shape=shape, optional=True)
+            _check_cuda_out(status, "status", (torch.uint8,), shape=shape, optional=True)
+        if shape[1]:
+            self._check(self._lib.magent_b200_get_reward_slots(self.game, g, _dptr(reward), _dptr(status)),
+                        "get_reward_slots")
+        return reward, status
+
+    def get_action_mask_slots(self, handle):
+        """bool (num_arenas, S, n_action): the legal-action mask (see get_action_mask) in the stable slot layout; all
+        False in vacant slots and for dead, un-culled agents.  The array is a cached receive buffer: valid until the next
+        call."""
+        g = self._hv(handle)
+        buf = self._host_view((g, "mask_slots"), self._slot_shape(handle) + (self.action_space[g][0],), np.uint8)
+        if buf.size:
+            self._check(self._lib.magent_b200_get_action_mask_slots(self.game, g, buf.ctypes.data),
+                        "get_action_mask_slots")
+        return buf.view(np.bool_)
+
+    def get_action_mask_slots_torch(self, handle, out=None):
+        """the slot-ordered legal-action mask (see get_action_mask_slots) written straight into a CUDA torch.bool tensor
+        (num_arenas, S, n_action), without waiting for the device.
+
+        out: a caller-owned contiguous CUDA tensor of that shape, torch.bool or torch.uint8; needed to record the call
+        into a CUDA graph (capture_graph), since the call then allocates nothing once a first call has run."""
+        import torch
+        g = self._hv(handle)
+        shape = self._slot_shape(handle) + (self.action_space[g][0],)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.uint8, device="cuda")
+        else:
+            _check_cuda_out(out, "out", (torch.bool, torch.uint8), shape=shape)
+        if out.numel():
+            self._check(self._lib.magent_b200_get_action_mask_slots(self.game, g, ctypes.c_void_p(out.data_ptr())),
+                        "get_action_mask_slots")
+        return out.view(torch.bool)
+
     def get_counters(self):
         """int64 event counters accumulated on the device since construction"""
         buf = (ctypes.c_longlong * 16)()
