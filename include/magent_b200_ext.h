@@ -244,7 +244,10 @@ int magent_b200_set_host_threads(int n);       /* 0 = default (usable cores, at 
  * does not fit in shared memory).  A negative value or obs_tile > 2 is refused: env_config_game returns -1 and nothing
  * changes.  env_get_info(game, -1, "obs_override", int[3]) reads the three keys back.
  * env_get_info(game, -1, "obs_launch", int[8]) reports the last obs_render_kernel launch of the game: {sizeof(T), NIT,
- * turn, agents per tile, grid, chunk, tiles, view and feature buffers both 16-byte aligned}, zeros before the first. */
+ * turn, agents per tile, grid, chunk, tiles, view and feature buffers both 16-byte aligned}, zeros before the first.
+ * env_get_info(game, -1, "step_launch", int[10]) reports the last step and clear_dead launches of the game, five ints
+ * each (step first): {mode (0 a CTA per arena, 1 the whole-grid team), grid, threads, dynamic shared-memory bytes, step
+ * scratch in shared memory}, zeros before the first. */
 
 #ifdef __cplusplus
 }

@@ -53,6 +53,10 @@ void launch_obs(Ctx *, const EngineDev *dE, const EngineDev &hE, const ObsArgs &
 // view and feature buffers both 16-byte aligned}; all zero before the first launch.  Declared weak like
 // launch_global_state: a backend without it loads, and the engine refuses the "obs_launch" info key.
 __attribute__((weak)) void obs_launch_report(const Ctx *, int out[8]);
+// the last step and cull launches of this context, five ints each (step first, then cull): {mode (0 CTA per arena,
+// 1 whole-grid team), grid, threads, dynamic shared-memory bytes, step scratch in shared memory (0 for the cull)}; all
+// zero before the first launch.  Weak like obs_launch_report: the engine refuses the "step_launch" info key without it.
+__attribute__((weak)) void step_launch_report(const Ctx *, int out[10]);
 // whole-map state of every arena into `out` ([A][H][W][state_channels], obs_phases.h state_compose_cell): float32, or
 // IEEE half (the float32 value rounded to nearest-even) when `half`.  A device buffer, 16-byte aligned.
 // Declared weak: the CUDA backend always defines it, a test backend may leave it out (the engine then refuses

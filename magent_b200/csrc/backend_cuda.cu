@@ -82,6 +82,7 @@ struct Ctx {
     // cudaFuncSetAttribute caches (per device: a context never changes device)
     struct ObsCfg { size_t smem = (size_t)-1; int ctas_per_sm = 1; } obs_cfg[12];
     int obs_last[8] = {0, 0, 0, 0, 0, 0, 0, 0};            // the last render launch (obs_launch_report)
+    int step_last[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};     // the last step and cull launches (step_launch_report)
     unsigned *obs_deal = nullptr;        // [sms + 1] render chunk counters; zero between launches (the kernel resets them)
     ObsCfg state_cfg[2];                 // global_state_kernel<float>, <__half>: CTAs per SM (smem 0 once queried)
     int restore_ctas_per_sm = 0;         // restore_kernel (0: not queried yet)
@@ -564,6 +565,12 @@ __global__ void __launch_bounds__(STEP_THREADS) cull_kernel_grid(const EngineDev
 
 static const int GRID_MODE_THRESHOLD = 32768;    // agents per arena above which the whole grid teams up
 
+// {mode (0 CTA per arena, 1 whole-grid team), grid, threads, dynamic smem bytes, scratch in smem} (step_launch_report)
+static void record_launch(int *out, int mode, int grid, int threads, int smem, int scratch_in_smem) {
+    const int report[5] = {mode, grid, threads, smem, scratch_in_smem};
+    memcpy(out, report, sizeof report);
+}
+
 // CTA-per-arena block size: the phases are latency-bound loops over the arena's agents, so with many
 // arenas we want many (small) CTAs resident per SM; with few arenas the single CTA should be wide.
 static int step_block_size(int sms, int arenas, int max_agents) {
@@ -589,6 +596,7 @@ void launch_step(Ctx *c, const EngineDev *dE, const EngineDev &hE, const StepArg
         void *args[] = {(void *)&dE, (void *)&s};
         CUDA_CHECK(cudaLaunchCooperativeKernel((const void *)step_kernel_grid, dim3(grid), dim3(GRID_THREADS), args, 0, c->stream));
         post_launch("step_kernel_grid");
+        record_launch(c->step_last, 1, grid, GRID_THREADS, 0, 0);
     } else {
         // scratch in shared memory whenever one arena's scratch fits: fewer, wider CTAs (latency per phase drops
         // from HBM/L2 round trips to LDS), and the concurrently active arenas stay L2-resident
@@ -612,6 +620,7 @@ void launch_step(Ctx *c, const EngineDev *dE, const EngineDev &hE, const StepArg
         int grid = hE.A < per_sm * g_sms ? hE.A : per_sm * g_sms;
         step_kernel_cta<<<grid, threads, smem, c->stream>>>(dE, S, in_smem ? 1 : 0);
         post_launch("step_kernel_cta");
+        record_launch(c->step_last, 0, grid, threads, (int)smem, in_smem ? 1 : 0);
     }
 }
 
@@ -623,6 +632,7 @@ void launch_cull(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curm
         void *args[] = {(void *)&dE, (void *)&curmask};
         CUDA_CHECK(cudaLaunchCooperativeKernel((const void *)cull_kernel_grid, dim3(grid), dim3(GRID_THREADS), args, 0, c->stream));
         post_launch("cull_kernel_grid");
+        record_launch(c->step_last + 5, 1, grid, GRID_THREADS, 0, 0);
     } else {
         int grid = hE.A < 8 * g_sms ? hE.A : 8 * g_sms;
         // measurement knob: MAGENT_B200_CULL_THREADS overrides the block size
@@ -633,6 +643,7 @@ void launch_cull(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curm
         if (cull_pref >= 32 && cull_pref <= STEP_THREADS) threads = cull_pref & ~31;
         cull_kernel_cta<<<grid, threads, 0, c->stream>>>(dE, curmask);
         post_launch("cull_kernel_cta");
+        record_launch(c->step_last + 5, 0, grid, threads, 0, 0);
     }
 }
 
@@ -1889,6 +1900,7 @@ void launch_obs(Ctx *c, const EngineDev *, const EngineDev &hE, const ObsArgs &O
 }
 
 void obs_launch_report(const Ctx *c, int out[8]) { memcpy(out, c->obs_last, sizeof c->obs_last); }
+void step_launch_report(const Ctx *c, int out[10]) { memcpy(out, c->step_last, sizeof c->step_last); }
 
 // ------------------------------------------------------------------------------------------------
 // global state (magent_b200_get_global_state): state_compose_cell of every map cell of every arena, [A][H][W][C] in T.

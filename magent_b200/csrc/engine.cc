@@ -1824,6 +1824,12 @@ int Engine::get_info(int group, const char *name, void *void_buffer) {         /
         if (bx_) be::obs_launch_report(bx_, ib);
         return 0;
     }
+    if (strequ(name, "step_launch")) {                  // extension: shape of this engine's last step and cull launches
+        if (!be::step_launch_report) return refuse("the %s backend does not report its step launches", be::name());
+        for (int i = 0; i < 10; ++i) ib[i] = 0;
+        if (bx_) be::step_launch_report(bx_, ib);
+        return 0;
+    }
     if (strequ(name, "state_space")) {                  // extension: per-arena shape of magent_b200_get_global_state
         ib[0] = H_; ib[1] = W_; ib[2] = state_channels();               // fixed: no counts needed, nothing to wait for
         return 0;

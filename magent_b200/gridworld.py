@@ -959,6 +959,14 @@ class GridWorld(Environment):
         keys = ("elem_bytes", "nit", "turn", "tile_agents", "grid", "chunk", "tiles", "aligned")
         return dict(zip(keys, (int(v) for v in buf)))
 
+    def _get_step_launch(self):
+        """the last step and cull launches of this engine: two dicts(mode (0 a CTA per arena, 1 the whole-grid team),
+        grid, threads, smem, scratch_in_smem); all zero before the first launch"""
+        buf = np.zeros((10,), dtype=np.int32)
+        self._check(self._lib.env_get_info(self.game, -1, b"step_launch", buf.ctypes.data), "step_launch")
+        keys = ("mode", "grid", "threads", "smem", "scratch_in_smem")
+        return tuple(dict(zip(keys, (int(v) for v in buf[k:k + 5]))) for k in (0, 5))
+
     def launch_count(self):
         """number of kernels this library has launched in this process"""
         return int(self._lib.magent_b200_launch_count())
