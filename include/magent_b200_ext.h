@@ -160,6 +160,28 @@ int magent_b200_get_reward_slots(EnvHandle game, GroupHandle group, float *rewar
  * and counted in the d2h figure.  Returns -1, sets magent_b200_last_error and writes nothing for a bad group handle, a
  * NULL mask, or a backend without the kernel. */
 int magent_b200_get_action_mask_slots(EnvHandle game, GroupHandle group, unsigned char *mask);
+/* The mean neighbour action and the nearest visible neighbours in the [arena, slot] layout of magent_b200_get_slots.
+ * S = slot_space(group), S_of = slot_space(of) (env_get_info "slot_space"), A = num_arenas; slot_row and row_slot are the
+ * maps magent_b200_get_slots serves at the same moment, row_slot_of those of group `of`.
+ *   get_mean_action_slots: mean float32 [A][S][n_action(of)], count int32 [A][S] (may be NULL).  An occupied slot (a, s)
+ *     holds, bit for bit, the row magent_b200_get_mean_action gives row slot_row[a][s] (a dead, un-culled agent's row is
+ *     zero and its count 0, as there); a vacant slot a +0.0 row and count 0.
+ *   get_neighbours_slots: idx int32 [A][S][k], rel int32 [A][S][k][2] and count int32 [A][S] (rel and count may be
+ *     NULL), 1 <= k <= 32.  An occupied slot holds the row magent_b200_get_neighbours gives row slot_row[a][s], with every
+ *     used idx entry the neighbour's flat slot row_slot_of[its row] = a * S_of + slot_of instead of its row: gather
+ *     slot-ordered features of `of` with hid_s.view(A * S_of, d)[idx.clamp(min=0)].  rel and count are the row call's;
+ *     unused entries are -1.  A vacant slot holds -1 everywhere and count 0.  Unlike row indices, these stay valid for the
+ *     whole episode: after a clear_dead one may point at a vacant slot (its agent was culled), never at another agent.
+ * Neither call waits for the agent counts, whatever the pointer kind.  Both CUDA device pointers: no synchronisation and,
+ * once a first call has sized the engine's tables, no allocation, so the calls can be recorded into a CUDA graph, also
+ * after a restore from a device src inside the graph.  Host pointers: computed into device staging and copied back,
+ * counted in the d2h figure (exactly the bytes asked for).  They cover every arena whatever magent_b200_select_arena
+ * says; S == 0 writes nothing.  Returns -1, sets magent_b200_last_error and writes nothing for a bad `group` or `of`
+ * handle, k out of range, a NULL mean / idx, pointers that mix host and CUDA device memory, a view too large to order
+ * its cells by an int key (as magent_b200_get_neighbours refuses it), or a backend without the kernel. */
+int magent_b200_get_mean_action_slots(EnvHandle game, GroupHandle group, GroupHandle of, float *mean, int *count);
+int magent_b200_get_neighbours_slots(EnvHandle game, GroupHandle group, GroupHandle of, int k, int *idx, int *rel,
+                                     int *count);
 /* compact observation hand-off (SURVEY.md 8f rank 2): same call, layout and pointer rules as env_get_observation
  * (reference src/runtime_api.h:35), but every element is an IEEE binary16 = the float32 value rounded to
  * nearest-even.  buffer[0] = view [n][view_h][view_w][n_channel], buffer[1] = feature [n][feature_size];

@@ -72,6 +72,8 @@ EXT_SIGNATURES = {
     "magent_b200_set_action_slots": ([_vp, ctypes.c_int, _vp], ctypes.c_int),
     "magent_b200_get_reward_slots": ([_vp, ctypes.c_int, _vp, _vp], ctypes.c_int),
     "magent_b200_get_action_mask_slots": ([_vp, ctypes.c_int, _vp], ctypes.c_int),
+    "magent_b200_get_mean_action_slots": ([_vp, ctypes.c_int, ctypes.c_int, _vp, _vp], ctypes.c_int),
+    "magent_b200_get_neighbours_slots": ([_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp], ctypes.c_int),
     "magent_b200_get_observation_f16": ([_vp, ctypes.c_int, ctypes.POINTER(_vp)], ctypes.c_int),
     "magent_b200_get_global_state": ([_vp, _vp, ctypes.c_int], ctypes.c_int),
     "magent_b200_snapshot_arenas": ([_vp], ctypes.c_int),

@@ -127,6 +127,18 @@ __attribute__((weak)) void launch_reward_slots(Ctx *, const EngineDev *dE, const
                                                unsigned curmask, int group, int S, float *reward, unsigned char *status);
 __attribute__((weak)) void launch_action_mask_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
                                                     unsigned curmask, int group, int S, unsigned char *mask);
+// The mean action and the neighbours of `group` in slot order (slot_phases.h, the device-side offsets decide the rows; all
+// buffers are device buffers).  launch_mean_action_slots: mean [A][S][n_action(of)] and, unless null, count [A][S], the
+// rows launch_mean_action writes for the row in each slot, +0.0 and 0 where no row is.  launch_neighbours_slots: idx
+// [A][S][k] and, unless null, rel [A][S][k][2] and count [A][S], the rows launch_neighbours writes for the row in each
+// slot with every stored idx entry the neighbour's a * S_of + slot in group `of` (S_of = of's slot space) instead of its
+// row; all -1 and count 0 where no row is.  `lut` as for launch_neighbours.  Weak like launch_slots: the engine refuses
+// the calls without them.
+__attribute__((weak)) void launch_mean_action_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
+                                                    unsigned curmask, int group, int of, int S, float *mean, int *count);
+__attribute__((weak)) void launch_neighbours_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
+                                                   const NbrCell *lut, unsigned curmask, int group, int of, int k, int S,
+                                                   int S_of, int *idx, int *rel, int *count);
 // clear_dead: asynchronous read-back of the [G][A+1] offset table (launch_offsets) into page-locked memory
 void counts_fetch_begin(Ctx *, const int *dev_off, size_t n_ints);
 const int *counts_fetch_wait(Ctx *);     // blocks until the fetch has landed; valid until the next counts_fetch_begin

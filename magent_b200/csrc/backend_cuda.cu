@@ -48,7 +48,7 @@ static std::atomic<long long> g_launches{0};       // instrumentation only (mage
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize belongs to (function, device), not to an engine: it is only ever raised,
 // under a lock, so that a second engine with a smaller need cannot pull it from under the first
-enum { ATTR_STEP = 0, ATTR_OBS0 = 1, ATTR_MEAN = 1 + 12, ATTR_N, ATTR_MAX_DEVICES = 64 };
+enum { ATTR_STEP = 0, ATTR_OBS0 = 1, ATTR_MEAN = 1 + 12, ATTR_MEAN_SLOTS, ATTR_N, ATTR_MAX_DEVICES = 64 };
 static std::mutex g_attr_mu;
 static size_t g_attr_smem[ATTR_MAX_DEVICES][ATTR_N];
 template <class K>
@@ -75,8 +75,9 @@ struct Ctx {
     float *mm_pad = nullptr; size_t mm_pad_n = 0; int mm_stride = 0;
     // per-observer headers of the render kernel
     int4 *obs_hdr = nullptr; size_t obs_hdr_n = 0;
-    // slot-ordered observations (launch_obs_slots): the [A][S] slot -> row scratch (launch_action_mask_slots uses it
-    // too), and the render's count bound ([A + 1] words of INT_MAX)
+    // slot-ordered observations (launch_obs_slots): the [A][S] slot -> row scratch (launch_action_mask_slots,
+    // launch_mean_action_slots and launch_neighbours_slots use it too), and the render's count bound ([A + 1] words of
+    // INT_MAX)
     int *obs_slot_row = nullptr; size_t obs_slot_row_n = 0;
     int *obs_slot_bound = nullptr; size_t obs_slot_bound_n = 0;
     // cudaFuncSetAttribute caches (per device: a context never changes device)
@@ -884,27 +885,46 @@ static_assert(MEAN_OBS / MEAN_WARPS <= 32, "a warp's observers are loaded one pe
 // The kernel is latency-bound (a kind -> occ -> act chain per observer), so resident warps matter: five CTAs per SM
 // leave it 44 registers without spills (58 unbounded, four CTAs; six CTAs spill).  DESIGN.md §5 has the numbers.
 
-__global__ void __launch_bounds__(MEAN_THREADS, 5) mean_action_kernel(const EngineDev *gE, unsigned curmask, int g, int of,
-                                                                  float *mean, int *count, int n_total,
-                                                                  int chunks_per_arena) {
-    __shared__ EngineDev sE;
-    __shared__ int n_in_s;
-    extern __shared__ __align__(16) unsigned char mean_smem[];
-    load_engine(&sE, gE);
-    const EngineDev &E = sE;
+// Who observer v of a CTA of the mean-action and neighbours kernels is, by a compile-time policy.  Rows (SLOTS false:
+// mean_action_kernel, neighbours_kernel): row v of arena a in the group's order.  Slots (SLOTS true: the *_slots kernels):
+// slot v of arena a, whose row slot_row (arena a's [S] block of slots_kernel's map) names; a vacant slot loads as the
+// dead placeholder, which takes the dead observer's path (zero row, no neighbours).  o0 is the arena's first row.  A
+// slot's lane keeps its row in arena i (< 2^24, code_index), its heading and its dead bit in one word, mine.code =
+// i << 8 | dir << 1 | dead: the slot's cell code has to be held through the walk, where a row's is recomputed from v,
+// and a lane word less keeps neighbours_slots_kernel free of spills at five CTAs per SM.
+template <bool SLOTS>
+__device__ __forceinline__ void nbr_cta_load(const EngineDev &E, unsigned curmask, int a, int g, int o0,
+                                             const int *slot_row, int v, NbrObserver &mine) {
+    if (!SLOTS) { mine = nbr_observer(E, curmask, a, g, v); return; }
+    const int r = slot_row[v];
+    if (r < 0) { mine.code = FLAG_DEAD; return; }
+    mine = nbr_observer(E, curmask, a, g, r - o0);
+    mine.code = (r - o0) << 8 | mine.dir << 1 | (mine.flags & FLAG_DEAD);
+}
+// the heading, cell code (which nbr_at and nbr_nearest_at exclude) and flags of observer v, loaded by lane u of the warp
+template <bool SLOTS>
+__device__ __forceinline__ void nbr_cta_take(int g, int v, const NbrObserver &mine, int u, NbrObserver &o) {
+    if (SLOTS) {
+        const int w = __shfl_sync(0xffffffffu, mine.code, u);
+        o.dir = (w >> 1) & 3; o.code = code_make(g, (int)((unsigned)w >> 8)); o.flags = (unsigned char)(w & FLAG_DEAD);
+        return;
+    }
+    o.dir = __shfl_sync(0xffffffffu, mine.dir, u); o.code = code_make(g, v);
+    o.flags = (unsigned char)__shfl_sync(0xffffffffu, (int)mine.flags, u);
+}
+
+// One CTA of the mean-action kernels: observers c0 .. c0 + cta_cnt - 1 of arena a (nbr_cta_load), the row of observer v
+// written at out0 + v.  The view LUT and the warps' histograms live in `smem`.
+template <bool SLOTS>
+__device__ __forceinline__ void mean_action_cta(const EngineDev &E, unsigned curmask, int g, int of, float *mean,
+                                                int *count, int a, int c0, int cta_cnt, int o0, const int *slot_row,
+                                                int out0, unsigned char *smem, int &n_in_s) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int a = blockIdx.x / chunks_per_arena;
-    const int c0 = (blockIdx.x - a * chunks_per_arena) * MEAN_OBS;
-    const int *off = E.off + (size_t)g * (E.A + 1);
-    const int o0 = off[a];
-    int cta_cnt = min(MEAN_OBS, off[a + 1] - o0 - c0);
-    cta_cnt = min(cta_cnt, n_total - (o0 + c0));                 // never beyond the caller's buffers
-    if (cta_cnt <= 0) return;
     const GroupDev &G = E.grp[g];
     const int na = E.grp[of].n_action;
     const int lut_stride = G.view_count;
     // lut[k] = {offset of the map cell in the padded planes from the observer's own cell, dx | dy << 16}
-    int2 *lut = (int2 *)mean_smem;
+    int2 *lut = (int2 *)smem;
     int *hist = (int *)(lut + (E.turn_mode ? 4 : 1) * lut_stride) + warp * na;
     if (warp == 0) {                                          // compact the view mask, order-preserving
         const int cells = G.view_w * G.view_h;
@@ -931,14 +951,13 @@ __global__ void __launch_bounds__(MEAN_THREADS, 5) mean_action_kernel(const Engi
     const int n_mine = cta_cnt > warp ? (cta_cnt - warp + MEAN_WARPS - 1) / MEAN_WARPS : 0;
     NbrObserver mine;                                         // lane u: observer c0 + warp + MEAN_WARPS * u
     mine.x = mine.y = 0; mine.dir = DIR_NORTH; mine.code = 0; mine.flags = FLAG_DEAD;
-    if (lane < n_mine) mine = nbr_observer(E, curmask, a, g, c0 + warp + MEAN_WARPS * lane);
+    if (lane < n_mine) nbr_cta_load<SLOTS>(E, curmask, a, g, o0, slot_row, c0 + warp + MEAN_WARPS * lane, mine);
     const unsigned char *kplane = E.kind + (long)a * E.kplane;
     for (int u = 0; u < n_mine; ++u) {
         const int i = c0 + warp + MEAN_WARPS * u;
         NbrObserver o;
         o.x = __shfl_sync(0xffffffffu, mine.x, u); o.y = __shfl_sync(0xffffffffu, mine.y, u);
-        o.dir = __shfl_sync(0xffffffffu, mine.dir, u); o.code = code_make(g, i);
-        o.flags = (unsigned char)__shfl_sync(0xffffffffu, (int)mine.flags, u);
+        nbr_cta_take<SLOTS>(g, i, mine, u, o);
         for (int k = lane; k < na; k += 32) hist[k] = 0;
         __syncwarp();
         int cnt = 0;
@@ -963,11 +982,29 @@ __global__ void __launch_bounds__(MEAN_THREADS, 5) mean_action_kernel(const Engi
             cnt = __reduce_add_sync(0xffffffffu, cnt);
         }
         __syncwarp();
-        float *row = mean + (size_t)(o0 + i) * na;
+        float *row = mean + (size_t)(out0 + i) * na;
         for (int k = lane; k < na; k += 32) row[k] = nbr_mean(hist[k], cnt);
-        if (count && lane == 0) count[o0 + i] = cnt;
+        if (count && lane == 0) count[out0 + i] = cnt;
         __syncwarp();                                         // the histogram is read before the next observer clears it
     }
+}
+
+__global__ void __launch_bounds__(MEAN_THREADS, 5) mean_action_kernel(const EngineDev *gE, unsigned curmask, int g, int of,
+                                                                  float *mean, int *count, int n_total,
+                                                                  int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    __shared__ int n_in_s;
+    extern __shared__ __align__(16) unsigned char mean_smem[];
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int a = blockIdx.x / chunks_per_arena;
+    const int c0 = (blockIdx.x - a * chunks_per_arena) * MEAN_OBS;
+    const int *off = E.off + (size_t)g * (E.A + 1);
+    const int o0 = off[a];
+    int cta_cnt = min(MEAN_OBS, off[a + 1] - o0 - c0);
+    cta_cnt = min(cta_cnt, n_total - (o0 + c0));                 // never beyond the caller's buffers
+    if (cta_cnt <= 0) return;
+    mean_action_cta<false>(E, curmask, g, of, mean, count, a, c0, cta_cnt, o0, nullptr, o0, mean_smem, n_in_s);
 }
 
 void launch_mean_action(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group, int of,
@@ -999,35 +1036,37 @@ constexpr int NBR_THREADS = 256, NBR_OBS = 128, NBR_ROUNDS = 4;
 constexpr int NBR_WARPS = NBR_THREADS / 32;
 static_assert(NBR_OBS / NBR_WARPS <= 32, "a warp's observers are loaded one per lane");
 
-__global__ void __launch_bounds__(NBR_THREADS, 5) neighbours_kernel(const EngineDev *gE, const NbrCell *lut,
-                                                                    unsigned curmask, int g, int of, int k, int *idx,
-                                                                    int *rel, int *count, int n_total,
-                                                                    int chunks_per_arena) {
-    __shared__ EngineDev sE;
-    load_engine(&sE, gE);
-    const EngineDev &E = sE;
+// The idx entry of neighbour j (index j of group `of` in arena a): its row, base + j, or (SLOTS) its flat slot
+// a * S_of + slot, looked up through its id as slots_kernel looks up a row's (slot_phases.h slot_flat).  Only stored
+// entries are translated: two dependent loads per stored neighbour.
+template <bool SLOTS>
+__device__ __forceinline__ int nbr_cta_index(const EngineDev &E, unsigned curmask, int a, int of, int base, int j,
+                                             const SlotDev *T, int S_of) {
+    if (!SLOTS) return base + j;
+    return slot_flat(T->tab, T->id_cap, a, cur_soa(E, curmask, of).id[gidx(E, a, of, j)], S_of);
+}
+
+// One CTA of the neighbours kernels: observers c0 .. c0 + cta_cnt - 1 of arena a (nbr_cta_load), the row of observer v
+// written at out0 + v.
+template <bool SLOTS>
+__device__ __forceinline__ void neighbours_cta(const EngineDev &E, const NbrCell *lut, unsigned curmask, int g, int of,
+                                               int k, int *idx, int *rel, int *count, int a, int c0, int cta_cnt, int o0,
+                                               const int *slot_row, int out0, const SlotDev *T, int S_of) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int a = blockIdx.x / chunks_per_arena;
-    const int c0 = (blockIdx.x - a * chunks_per_arena) * NBR_OBS;
-    const int o0 = E.off[(size_t)g * (E.A + 1) + a];
-    int cta_cnt = min(NBR_OBS, E.off[(size_t)g * (E.A + 1) + a + 1] - o0 - c0);
-    cta_cnt = min(cta_cnt, n_total - (o0 + c0));                 // never beyond the caller's buffers
-    if (cta_cnt <= 0) return;
     const int base = E.off[(size_t)of * (E.A + 1) + a];          // row of j = base + j in `of`'s concatenation
     const int n_in = E.grp[g].view_count;
     const int n_mine = cta_cnt > warp ? (cta_cnt - warp + NBR_WARPS - 1) / NBR_WARPS : 0;
     NbrObserver mine;                                             // lane u: observer c0 + warp + NBR_WARPS * u
     mine.x = mine.y = 0; mine.dir = DIR_NORTH; mine.code = 0; mine.flags = FLAG_DEAD;
-    if (lane < n_mine) mine = nbr_observer(E, curmask, a, g, c0 + warp + NBR_WARPS * lane);
+    if (lane < n_mine) nbr_cta_load<SLOTS>(E, curmask, a, g, o0, slot_row, c0 + warp + NBR_WARPS * lane, mine);
     const unsigned char *kplane = E.kind + (long)a * E.kplane;
     const unsigned lower = (1u << lane) - 1u;
     for (int u = 0; u < n_mine; ++u) {
         const int i = c0 + warp + NBR_WARPS * u;
         NbrObserver o;
         o.x = __shfl_sync(0xffffffffu, mine.x, u); o.y = __shfl_sync(0xffffffffu, mine.y, u);
-        o.dir = __shfl_sync(0xffffffffu, mine.dir, u); o.code = code_make(g, i);
-        o.flags = (unsigned char)__shfl_sync(0xffffffffu, (int)mine.flags, u);
-        const size_t row = (size_t)(o0 + i) * k;
+        nbr_cta_take<SLOTS>(g, i, mine, u, o);
+        const size_t row = (size_t)(out0 + i) * k;
         int found = 0;
         if (!(o.flags & FLAG_DEAD)) {
             const unsigned char *kp = kplane + (long)(o.y + E.kpad) * E.kw + o.x + E.kpad;
@@ -1049,7 +1088,7 @@ __global__ void __launch_bounds__(NBR_THREADS, 5) neighbours_kernel(const Engine
                     const unsigned hits = __ballot_sync(0xffffffffu, j >= 0);
                     const int slot = found + __popc(hits & lower);
                     if (j >= 0 && slot < k) {
-                        idx[row + slot] = base + j;
+                        idx[row + slot] = nbr_cta_index<SLOTS>(E, curmask, a, of, base, j, T, S_of);
                         if (rel) { rel[2 * (row + slot)] = cell >> 16; rel[2 * (row + slot) + 1] = cell & 0xffff; }
                     }
                     found += __popc(hits);
@@ -1060,8 +1099,24 @@ __global__ void __launch_bounds__(NBR_THREADS, 5) neighbours_kernel(const Engine
             idx[row + s] = -1;
             if (rel) { rel[2 * (row + s)] = -1; rel[2 * (row + s) + 1] = -1; }
         }
-        if (count && lane == 0) count[o0 + i] = found;
+        if (count && lane == 0) count[out0 + i] = found;
     }
+}
+
+__global__ void __launch_bounds__(NBR_THREADS, 5) neighbours_kernel(const EngineDev *gE, const NbrCell *lut,
+                                                                    unsigned curmask, int g, int of, int k, int *idx,
+                                                                    int *rel, int *count, int n_total,
+                                                                    int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int a = blockIdx.x / chunks_per_arena;
+    const int c0 = (blockIdx.x - a * chunks_per_arena) * NBR_OBS;
+    const int o0 = E.off[(size_t)g * (E.A + 1) + a];
+    int cta_cnt = min(NBR_OBS, E.off[(size_t)g * (E.A + 1) + a + 1] - o0 - c0);
+    cta_cnt = min(cta_cnt, n_total - (o0 + c0));                 // never beyond the caller's buffers
+    if (cta_cnt <= 0) return;
+    neighbours_cta<false>(E, lut, curmask, g, of, k, idx, rel, count, a, c0, cta_cnt, o0, nullptr, o0, nullptr, 0);
 }
 
 void launch_neighbours(Ctx *c, const EngineDev *dE, const EngineDev &hE, const NbrCell *lut, unsigned curmask, int group,
@@ -2642,6 +2697,21 @@ void launch_reward_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, const
     post_launch("reward_slots_kernel");
 }
 
+// the [A][S] slot -> row map of `group` in c->obs_slot_row (grown outside a capture only)
+static void slot_rows_scratch(Ctx *c, const EngineDev &hE, const SlotDev *T, unsigned curmask, int group, int S,
+                              const char *what) {
+    const size_t n = (size_t)hE.A * S;
+    if (n > c->obs_slot_row_n) {
+        no_capture(c, what);
+        grow_dev(c, c->obs_slot_row, c->obs_slot_row_n, n);
+    }
+    const GroupDev &D = hE.grp[group];
+    slots_kernel<<<(unsigned)hE.A, SLOT_THREADS, 0, c->stream>>>(hE.off + (size_t)group * (hE.A + 1),
+                                                                 D.soa[(curmask >> group) & 1u].id, D.cap, T, hE.A, S,
+                                                                 nullptr, c->obs_slot_row, 0x7fffffff);
+    post_launch("slots_kernel");
+}
+
 // Mask: slots_kernel writes the [A][S] slot -> row map into the scratch of the slot-ordered observation, then
 // action_mask_slots_kernel takes MASK_THREADS consecutive slots of one arena per CTA, so an arena gets several CTAs
 // whatever its population (a one-arena batch is not one CTA).  It is action_mask_kernel with the lanes' agents looked up
@@ -2689,19 +2759,79 @@ void launch_action_mask_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, 
     const int na = hE.grp[group].n_action;
     const size_t smem = (size_t)MASK_THREADS * na + 16;
     if (smem + sizeof(EngineDev) > 48 * 1024) mg::fatal("action mask: %d actions per agent are more than the kernels hold", na);
-    if (n > c->obs_slot_row_n) {
-        no_capture(c, "growing the slot table of the slot-ordered action mask");
-        grow_dev(c, c->obs_slot_row, c->obs_slot_row_n, n);
-    }
-    const GroupDev &D = hE.grp[group];
-    slots_kernel<<<(unsigned)hE.A, SLOT_THREADS, 0, c->stream>>>(hE.off + (size_t)group * (hE.A + 1),
-                                                                 D.soa[(curmask >> group) & 1u].id, D.cap, T, hE.A, S,
-                                                                 nullptr, c->obs_slot_row, 0x7fffffff);
-    post_launch("slots_kernel");
+    slot_rows_scratch(c, hE, T, curmask, group, S, "growing the slot table of the slot-ordered action mask");
     const int cps = (S + MASK_THREADS - 1) / MASK_THREADS;
     action_mask_slots_kernel<<<(unsigned)((size_t)hE.A * cps), MASK_THREADS, smem, c->stream>>>(dE, curmask, group,
                                                                                                c->obs_slot_row, S, mask, cps);
     post_launch("action_mask_slots_kernel");
+}
+
+// Mean action and neighbours in slot order (magent_b200_get_mean_action_slots, _get_neighbours_slots): slots_kernel
+// writes the group's [A][S] slot -> row map into the same scratch as for the mask, then the kernels run the CTAs of
+// mean_action_kernel and neighbours_kernel under the slot policy (nbr_cta_load): a CTA takes MEAN_OBS / NBR_OBS
+// consecutive slots of one arena, so a one-arena batch still gets many CTAs, and writes its rows at a * S + slot, one
+// contiguous range.  A vacant slot's lane holds the dead placeholder, so the dead-observer path writes its zero / -1 row.
+__global__ void __launch_bounds__(MEAN_THREADS, 5) mean_action_slots_kernel(const EngineDev *gE, unsigned curmask, int g,
+                                                                        int of, const int *slot_row, int S, float *mean,
+                                                                        int *count, int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    __shared__ int n_in_s;
+    extern __shared__ __align__(16) unsigned char mean_smem[];
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int a = blockIdx.x / chunks_per_arena;
+    const int c0 = (blockIdx.x - a * chunks_per_arena) * MEAN_OBS;
+    const int o0 = E.off[(size_t)g * (E.A + 1) + a];
+    mean_action_cta<true>(E, curmask, g, of, mean, count, a, c0, min(MEAN_OBS, S - c0), o0, slot_row + (size_t)a * S,
+                          a * S, mean_smem, n_in_s);
+}
+
+__global__ void __launch_bounds__(NBR_THREADS, 5) neighbours_slots_kernel(const EngineDev *gE, const NbrCell *lut,
+                                                                          unsigned curmask, int g, int of, int k,
+                                                                          const int *slot_row, int S, const SlotDev *T,
+                                                                          int S_of, int *idx, int *rel, int *count,
+                                                                          int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int a = blockIdx.x / chunks_per_arena;
+    const int c0 = (blockIdx.x - a * chunks_per_arena) * NBR_OBS;
+    const int o0 = E.off[(size_t)g * (E.A + 1) + a];
+    neighbours_cta<true>(E, lut, curmask, g, of, k, idx, rel, count, a, c0, min(NBR_OBS, S - c0), o0,
+                         slot_row + (size_t)a * S, a * S, T, S_of);
+}
+
+void launch_mean_action_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, const SlotDev *T, unsigned curmask,
+                              int group, int of, int S, float *mean, int *count) {
+    DeviceGuard guard(c);
+    const size_t n = (size_t)hE.A * S;
+    if (n == 0) return;
+    if (n > 0x7fffffff) mg::fatal("%zu slots are more than one launch covers (rows a * S + slot are ints)", n);
+    const size_t smem = (size_t)(hE.turn_mode ? 4 : 1) * hE.grp[group].view_count * sizeof(int2) +
+                        (size_t)MEAN_WARPS * hE.grp[of].n_action * sizeof(int);
+    if (smem + sizeof(EngineDev) + 64 > 227 * 1024)
+        mg::fatal("mean action: a view of %d cells is more than the kernel holds", hE.grp[group].view_count);
+    if (smem + sizeof(EngineDev) + 64 > 48 * 1024)
+        ensure_dynamic_smem(c->device, ATTR_MEAN_SLOTS, mean_action_slots_kernel, smem);
+    slot_rows_scratch(c, hE, T, curmask, group, S, "growing the slot table of the slot-ordered mean action");
+    const int cps = (S + MEAN_OBS - 1) / MEAN_OBS;
+    mean_action_slots_kernel<<<(unsigned)((size_t)hE.A * cps), MEAN_THREADS, smem, c->stream>>>(
+        dE, curmask, group, of, c->obs_slot_row, S, mean, count, cps);
+    post_launch("mean_action_slots_kernel");
+}
+
+void launch_neighbours_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, const SlotDev *T, const NbrCell *lut,
+                             unsigned curmask, int group, int of, int k, int S, int S_of, int *idx, int *rel,
+                             int *count) {
+    DeviceGuard guard(c);
+    const size_t n = (size_t)hE.A * S;
+    if (n == 0) return;
+    if (n > 0x7fffffff) mg::fatal("%zu slots are more than one launch covers (rows a * S + slot are ints)", n);
+    slot_rows_scratch(c, hE, T, curmask, group, S, "growing the slot table of the slot-ordered neighbours");
+    const int cps = (S + NBR_OBS - 1) / NBR_OBS;
+    neighbours_slots_kernel<<<(unsigned)((size_t)hE.A * cps), NBR_THREADS, 0, c->stream>>>(
+        dE, lut, curmask, group, of, k, c->obs_slot_row, S, T, S_of, idx, rel, count, cps);
+    post_launch("neighbours_slots_kernel");
 }
 
 }  // namespace be

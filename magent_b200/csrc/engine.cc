@@ -1565,6 +1565,47 @@ int Engine::get_action_mask_slots(int group, unsigned char *mask) {
     return 0;
 }
 
+// The mean neighbour action in slot order: float [A][S][n_action(of)] and int [A][S], zero in vacant slots
+int Engine::get_mean_action_slots(int group, int of, float *mean, int *count) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_mean_action_slots", group);
+    if (of < 0 || of >= G()) return refuse("invalid group handle %d for `of` in get_mean_action_slots", of);
+    if (!mean) return refuse("get_mean_action_slots needs a mean buffer");
+    if (!be::launch_mean_action_slots || !be::launch_restore_slots)
+        return refuse("the %s backend has no slot-ordered mean-action kernel", be::name());
+    const int mem = out_memory("get_mean_action_slots: mean and count", {mean, count});
+    if (mem < 0) return -1;
+    to_device();
+    const int S = slot_space(group);
+    const size_t n = (size_t)A_ * S;
+    read_back(mem == 1, {{mean, n * group_type_[of]->n_action * 4}, {count, n * 4}}, [&](void **to) {
+        be::launch_mean_action_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, of, S, (float *)to[0], (int *)to[1]);
+    });
+    return 0;
+}
+
+// The first k neighbours in slot order: int [A][S][k] flat slots a * S_of + slot of `of`, int [A][S][k][2] view cells
+// and int [A][S] counts, -1 and 0 in vacant slots
+int Engine::get_neighbours_slots(int group, int of, int k, int *idx, int *rel, int *count) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_neighbours_slots", group);
+    if (of < 0 || of >= G()) return refuse("invalid group handle %d for `of` in get_neighbours_slots", of);
+    if (k < 1 || k > 32) return refuse("get_neighbours_slots: k = %d is outside [1, 32]", k);
+    if (!idx) return refuse("get_neighbours_slots needs an idx buffer");
+    if (!be::launch_neighbours_slots || !be::launch_restore_slots)
+        return refuse("the %s backend has no slot-ordered neighbours kernel", be::name());
+    const int mem = out_memory("get_neighbours_slots: idx, rel and count", {idx, rel, count});
+    if (mem < 0) return -1;
+    to_device();
+    if (!nbr_key_fits_[group])
+        return refuse("get_neighbours_slots: the view of group %d is too large to order its cells by an int key", group);
+    const int S = slot_space(group);
+    const size_t n = (size_t)A_ * S, idx_bytes = n * k * 4;
+    read_back(mem == 1, {{idx, idx_bytes}, {rel, 2 * idx_bytes}, {count, n * 4}}, [&](void **to) {
+        be::launch_neighbours_slots(bx_, dE_, hE_, d_slot_dev_, d_nbr_lut_ + nbr_lut_base_[group], curmask_, group, of,
+                                    k, S, slot_space(of), (int *)to[0], (int *)to[1], (int *)to[2]);
+    });
+    return 0;
+}
+
 void Engine::step(int *done) {                                        // GridWorld.cc:456-631
     to_device();
     StepArgs S;

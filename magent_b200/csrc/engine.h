@@ -153,6 +153,12 @@ public:
     int set_action_slots(int group, const int *act);
     int get_reward_slots(int group, float *reward, unsigned char *status);
     int get_action_mask_slots(int group, unsigned char *mask);
+    // the mean action and the neighbours in slot order (S = slot_space(group), neither waits for the counts):
+    // get_mean_action's and get_neighbours's rows for the row in each slot, [A][S][...], with every used idx entry the
+    // neighbour's a * slot_space(of) + slot instead of its row; zero / -1 rows and count 0 in vacant slots.  -1 and the
+    // last error when refused.
+    int get_mean_action_slots(int group, int of, float *mean, int *count);
+    int get_neighbours_slots(int group, int of, int k, int *idx, int *rel, int *count);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads

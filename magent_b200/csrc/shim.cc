@@ -129,6 +129,13 @@ MG_API int magent_b200_get_reward_slots(EnvHandle game, GroupHandle group, float
 MG_API int magent_b200_get_action_mask_slots(EnvHandle game, GroupHandle group, unsigned char *mask) {
     return E(game)->get_action_mask_slots(group, mask);
 }
+MG_API int magent_b200_get_mean_action_slots(EnvHandle game, GroupHandle group, GroupHandle of, float *mean, int *count) {
+    return E(game)->get_mean_action_slots(group, of, mean, count);
+}
+MG_API int magent_b200_get_neighbours_slots(EnvHandle game, GroupHandle group, GroupHandle of, int k, int *idx, int *rel,
+                                            int *count) {
+    return E(game)->get_neighbours_slots(group, of, k, idx, rel, count);
+}
 MG_API int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **buffer) {
     E(game)->get_observation(group, buffer, 1);
     return 0;

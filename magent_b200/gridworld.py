@@ -892,6 +892,98 @@ class GridWorld(Environment):
                         "get_action_mask_slots")
         return out.view(torch.bool)
 
+    def get_mean_action_slots(self, handle, of=None):
+        """(mean float32 (num_arenas, S, n_action(of)), count int32 (num_arenas, S)): the mean neighbour action (see
+        get_mean_action) in the stable slot layout (see get_slots); a +0.0 row and count 0 in vacant slots.  Both arrays
+        are cached receive buffers: valid until the next call."""
+        g = self._hv(handle)
+        o = g if of is None else self._hv(of)
+        shape = self._slot_shape(handle)
+        mean = self._host_view((g, "mean_slots"), shape + (self.action_space[o][0],), np.float32)
+        count = self._host_view((g, "mean_count_slots"), shape, np.int32)
+        if count.size:
+            self._check(self._lib.magent_b200_get_mean_action_slots(self.game, g, o, mean.ctypes.data,
+                                                                    count.ctypes.data), "get_mean_action_slots")
+        return mean, count
+
+    def get_mean_action_slots_torch(self, handle, of=None, out=None):
+        """the slot-ordered mean neighbour action (see get_mean_action_slots) written straight into CUDA tensors, without
+        waiting for the device: (mean float32 (num_arenas, S, n_action(of)), count int32 (num_arenas, S)).
+
+        out: a caller-owned pair (mean, count) of contiguous CUDA tensors of those shapes and dtypes; needed to record
+        the call into a CUDA graph (capture_graph), since the call then allocates nothing once a first call has run.
+        count may be None: it is then not written, and None comes back in its place."""
+        import torch
+        g = self._hv(handle)
+        o = g if of is None else self._hv(of)
+        shape = self._slot_shape(handle)
+        mshape = shape + (self.action_space[o][0],)
+        if out is None:
+            mean = torch.empty(mshape, dtype=torch.float32, device="cuda")
+            count = torch.empty(shape, dtype=torch.int32, device="cuda")
+        else:
+            if not isinstance(out, (tuple, list)) or len(out) != 2:
+                raise ValueError("out must be a (mean, count) pair of CUDA tensors, count possibly None")
+            mean, count = out
+            _check_cuda_out(mean, "mean", (torch.float32,), shape=mshape)
+            _check_cuda_out(count, "count", (torch.int32,), shape=shape, optional=True)
+        if shape[1]:
+            self._check(self._lib.magent_b200_get_mean_action_slots(self.game, g, o, _dptr(mean), _dptr(count)),
+                        "get_mean_action_slots")
+        return mean, count
+
+    def get_neighbours_slots(self, handle, k, of=None):
+        """(idx int32 (num_arenas, S, k), rel int32 (num_arenas, S, k, 2), count int32 (num_arenas, S)): the nearest
+        visible neighbours (see get_neighbours) in the stable slot layout (see get_slots).  idx holds each neighbour's
+        flat slot a * S_of + slot in group `of` (S_of = get_slot_space(of)) instead of its row, so it stays valid for the
+        episode: after clear_dead it may name a vacant slot, never another agent.  Unused entries and vacant slots are
+        -1, with count 0.  The arrays are cached receive buffers: valid until the next call."""
+        g = self._hv(handle)
+        o = g if of is None else self._hv(of)
+        k = int(k)
+        if not 1 <= k <= 32:
+            raise ValueError("k must be in [1, 32], got %d" % k)
+        shape = self._slot_shape(handle)
+        idx = self._host_view((g, "nbr_idx_slots"), shape + (k,), np.int32)
+        rel = self._host_view((g, "nbr_rel_slots"), shape + (k, 2), np.int32)
+        count = self._host_view((g, "nbr_count_slots"), shape, np.int32)
+        if count.size:
+            self._check(self._lib.magent_b200_get_neighbours_slots(self.game, g, o, k, idx.ctypes.data, rel.ctypes.data,
+                                                                   count.ctypes.data), "get_neighbours_slots")
+        return idx, rel, count
+
+    def get_neighbours_slots_torch(self, handle, k, of=None, out=None):
+        """the slot-ordered nearest visible neighbours (see get_neighbours_slots) written straight into CUDA tensors,
+        without waiting for the device: (idx int32 (num_arenas, S, k), rel int32 (num_arenas, S, k, 2), count int32
+        (num_arenas, S)).  Gather slot-ordered features of group `of` with hid_s.view(-1, d)[idx.clamp(min=0)].
+
+        out: a caller-owned triple (idx, rel, count) of contiguous CUDA int32 tensors of those shapes; needed to record
+        the call into a CUDA graph (capture_graph), since the call then allocates nothing once a first call has run.  rel
+        and count may be None: they are then neither computed nor written (without count the kernel stops at the k-th
+        neighbour), and None comes back in their place."""
+        import torch
+        g = self._hv(handle)
+        o = g if of is None else self._hv(of)
+        k = int(k)
+        if not 1 <= k <= 32:
+            raise ValueError("k must be in [1, 32], got %d" % k)
+        shape = self._slot_shape(handle)
+        if out is None:
+            idx = torch.empty(shape + (k,), dtype=torch.int32, device="cuda")
+            rel = torch.empty(shape + (k, 2), dtype=torch.int32, device="cuda")
+            count = torch.empty(shape, dtype=torch.int32, device="cuda")
+        else:
+            if not isinstance(out, (tuple, list)) or len(out) != 3:
+                raise ValueError("out must be an (idx, rel, count) triple of CUDA tensors")
+            idx, rel, count = out
+            _check_cuda_out(idx, "idx", (torch.int32,), shape=shape + (k,))
+            _check_cuda_out(rel, "rel", (torch.int32,), shape=shape + (k, 2), optional=True)
+            _check_cuda_out(count, "count", (torch.int32,), shape=shape, optional=True)
+        if shape[1]:
+            self._check(self._lib.magent_b200_get_neighbours_slots(self.game, g, o, k, _dptr(idx), _dptr(rel),
+                                                                   _dptr(count)), "get_neighbours_slots")
+        return idx, rel, count
+
     def get_counters(self):
         """int64 event counters accumulated on the device since construction"""
         buf = (ctypes.c_longlong * 16)()
