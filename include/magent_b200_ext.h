@@ -39,7 +39,9 @@ int magent_b200_random_actions(EnvHandle game, GroupHandle group, void *unused, 
  *   attack  the aimed cell is on the board and holds an agent of another group, of the own group when the type has
  *           attack_in_group, or food (food_mode)
  * What other agents do in the same step is not anticipated.  A dead, un-culled agent has an all-zero row; an absorbed
- * absorber has no legal move (its turns and attacks are decided as for anyone else).  Returns -1 for a bad group handle.
+ * absorber has no legal move (its turns and attacks are decided as for anyone else).  Returns -1 for a bad group handle,
+ * and returns -1, sets magent_b200_last_error and writes nothing when 256 rows of n_action bytes do not fit the device's
+ * shared memory per block (on an H100: more than 881 actions; DESIGN.md §5 "Shared-memory limits").
  * Host pointer or CUDA device pointer.  With a device pointer: no synchronisation, no allocation, recordable into a CUDA
  * graph; rows are sized by the device-side counts, at most "num_bound" of them are written.  magent_b200_select_arena
  * does not apply. */
@@ -62,7 +64,10 @@ int magent_b200_random_legal_actions(EnvHandle game, GroupHandle group, unsigned
  * called after set_action it gives the actions just set.  A neighbour whose action is outside [0, n_action(of)) (added
  * since the last step, or an id the step ignores) is counted in count and in no bin: its row sums to less than 1.  A row
  * without neighbours is all zero; a dead, un-culled agent has an all-zero row and count 0.  Returns -1 for a bad `group`
- * or `of` handle, or when one pointer is host memory and the other a CUDA device pointer.  Both host pointers: the call
+ * or `of` handle, or when one pointer is host memory and the other a CUDA device pointer; and returns -1, sets
+ * magent_b200_last_error and writes nothing when the view LUT of `group` (one per heading in turn_mode) and eight
+ * histograms of n_action(of) ints do not fit the device's shared memory per block (on an H100 with 21 actions: circle
+ * views of radius 95 and more, 48 and more in turn_mode; DESIGN.md §5 "Shared-memory limits").  Both host pointers: the call
  * waits for the counts.  Both CUDA device pointers: no synchronisation, no allocation, recordable into a CUDA graph; rows
  * are sized by the device-side counts, at most "num_bound" of them are written.  magent_b200_select_arena does not
  * apply. */
@@ -158,7 +163,7 @@ int magent_b200_get_reward_slots(EnvHandle game, GroupHandle group, float *rewar
 /* mask uint8 [A][S][n_action]: an occupied slot's row is bit for bit the row magent_b200_get_action_mask gives its
  * agent's row (a dead, un-culled agent's row is all zero); a vacant slot's row is all zero.  Host pointer: copied back
  * and counted in the d2h figure.  Returns -1, sets magent_b200_last_error and writes nothing for a bad group handle, a
- * NULL mask, or a backend without the kernel. */
+ * NULL mask, a backend without the kernel, or an action space magent_b200_get_action_mask refuses. */
 int magent_b200_get_action_mask_slots(EnvHandle game, GroupHandle group, unsigned char *mask);
 /* The mean neighbour action and the nearest visible neighbours in the [arena, slot] layout of magent_b200_get_slots.
  * S = slot_space(group), S_of = slot_space(of) (env_get_info "slot_space"), A = num_arenas; slot_row and row_slot are the
@@ -178,7 +183,8 @@ int magent_b200_get_action_mask_slots(EnvHandle game, GroupHandle group, unsigne
  * counted in the d2h figure (exactly the bytes asked for).  They cover every arena whatever magent_b200_select_arena
  * says; S == 0 writes nothing.  Returns -1, sets magent_b200_last_error and writes nothing for a bad `group` or `of`
  * handle, k out of range, a NULL mean / idx, pointers that mix host and CUDA device memory, a view too large to order
- * its cells by an int key (as magent_b200_get_neighbours refuses it), or a backend without the kernel. */
+ * its cells by an int key (as magent_b200_get_neighbours refuses it), a mean action magent_b200_get_mean_action refuses
+ * for its shared memory, or a backend without the kernel. */
 int magent_b200_get_mean_action_slots(EnvHandle game, GroupHandle group, GroupHandle of, float *mean, int *count);
 int magent_b200_get_neighbours_slots(EnvHandle game, GroupHandle group, GroupHandle of, int k, int *idx, int *rel,
                                      int *count);

@@ -139,6 +139,14 @@ __attribute__((weak)) void launch_mean_action_slots(Ctx *, const EngineDev *dE, 
 __attribute__((weak)) void launch_neighbours_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
                                                    const NbrCell *lut, unsigned curmask, int group, int of, int k, int S,
                                                    int S_of, int *idx, int *rel, int *count);
+// Whether kernel `which` fits the device's shared memory for `group` (and, for the mean action, the histograms of group
+// `of`'s actions): its static shared memory plus what the view or the action space asks for, against the device's
+// opt-in limit per block (the default limit for the wire kernel, which does not opt in).  When it does not, *why (unless
+// null) says how many bytes it would need and what the device allows.  The engine asks before anything is staged or
+// written: it refuses the mask and mean-action calls with -1, and takes the dense path instead of the wire records.
+// Weak like launch_slots: without it nothing is refused (the test emulation has no shared-memory limit).
+enum { SMEM_ACTION_MASK, SMEM_ACTION_MASK_SLOTS, SMEM_MEAN_ACTION, SMEM_MEAN_ACTION_SLOTS, SMEM_OBS_WIRE };
+__attribute__((weak)) bool smem_fits(Ctx *, const EngineDev &hE, int which, int group, int of, std::string *why);
 // clear_dead: asynchronous read-back of the [G][A+1] offset table (launch_offsets) into page-locked memory
 void counts_fetch_begin(Ctx *, const int *dev_off, size_t n_ints);
 const int *counts_fetch_wait(Ctx *);     // blocks until the fetch has landed; valid until the next counts_fetch_begin

@@ -47,10 +47,13 @@ namespace be {
 static std::atomic<long long> g_launches{0};       // instrumentation only (magent_b200_launch_count)
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize belongs to (function, device), not to an engine: it is only ever raised,
-// under a lock, so that a second engine with a smaller need cannot pull it from under the first
-enum { ATTR_STEP = 0, ATTR_OBS0 = 1, ATTR_MEAN = 1 + 12, ATTR_MEAN_SLOTS, ATTR_N, ATTR_MAX_DEVICES = 64 };
+// under a lock, so that a second engine with a smaller need cannot pull it from under the first.  The same slots cache
+// each kernel's static shared memory.
+enum { ATTR_STEP = 0, ATTR_OBS0 = 1, ATTR_MEAN = 1 + 12, ATTR_MEAN_SLOTS, ATTR_MASK, ATTR_MASK_SLOTS, ATTR_WIRE,
+       ATTR_MINIMAP_SMALL, ATTR_N, ATTR_MAX_DEVICES = 64 };
 static std::mutex g_attr_mu;
 static size_t g_attr_smem[ATTR_MAX_DEVICES][ATTR_N];
+static size_t g_attr_static[ATTR_MAX_DEVICES][ATTR_N];      // static shared memory + 1 (0: not queried yet)
 template <class K>
 static void ensure_dynamic_smem(int device, int slot, K kernel, size_t smem) {
     std::lock_guard<std::mutex> lk(g_attr_mu);
@@ -59,11 +62,28 @@ static void ensure_dynamic_smem(int device, int slot, K kernel, size_t smem) {
     CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     have = smem;
 }
+// The kernel's own __shared__ variables as the compiler laid them out (cudaFuncAttributes::sharedSizeBytes: 6400 bytes
+// for the kernels that hold an EngineDev copy, 128 for the render and the wire kernel with CUDA 12.9), which a launch
+// adds to its dynamic shared memory.  Queried once per (kernel, device).
+template <class K>
+static size_t static_smem(int device, int slot, K kernel) {
+    std::lock_guard<std::mutex> lk(g_attr_mu);
+    size_t &have = g_attr_static[device % ATTR_MAX_DEVICES][slot];
+    if (!have) {
+        cudaFuncAttributes fa;
+        CUDA_CHECK(cudaFuncGetAttributes(&fa, kernel));
+        have = fa.sharedSizeBytes + 1;
+    }
+    return have - 1;
+}
 
 // Per-engine device context.  Everything the backend needs to remember between calls lives here, nothing in
 // process-global state: two engines on two devices (or on one) never see each other's scratch.
 struct Ctx {
     int device = 0, sms = 0;
+    // shared memory one block may use, static and dynamic together: by default, and with the opt-in of
+    // cudaFuncAttributeMaxDynamicSharedMemorySize (49152 and 232448 bytes on an H100)
+    size_t smem_block = 0, smem_optin = 0;
     cudaStream_t stream = nullptr;       // every kernel of this engine; created blocking, so work queued on the legacy
                                          // default stream (torch's default stream) stays ordered with it both ways
     cudaStream_t copy = nullptr;         // wire / dense DMA traffic (non-blocking; ordered by events)
@@ -109,6 +129,24 @@ struct Ctx {
     std::vector<cudaGraphExec_t> graphs;
 };
 
+// Where `dyn` bytes of dynamic shared memory put a launch of `kernel` (attribute slot `slot`), its static shared memory
+// added: 0 within the device's default per-block limit, 1 within the opt-in limit only, -1 beyond both.  *need: the total.
+template <class K>
+static int smem_band(const Ctx *c, int slot, K kernel, size_t dyn, size_t *need = nullptr) {
+    const size_t total = static_smem(c->device, slot, kernel) + dyn;
+    if (need) *need = total;
+    return total <= c->smem_block ? 0 : total <= c->smem_optin ? 1 : -1;
+}
+// Ready `kernel` for a launch with `dyn` bytes of dynamic shared memory: the opt-in when it needs it.  Beyond the opt-in
+// limit the process stops; the engine refuses such calls before they get here (smem_fits).
+template <class K>
+static void smem_prepare(const Ctx *c, int slot, K kernel, size_t dyn, const char *what) {
+    size_t need;
+    const int band = smem_band(c, slot, kernel, dyn, &need);
+    if (band < 0) mg::fatal("%s: %zu bytes of shared memory, more than the %zu one block may use", what, need, c->smem_optin);
+    if (band > 0) ensure_dynamic_smem(c->device, slot, kernel, dyn);
+}
+
 static void no_capture(const Ctx *c, const char *what) {
     if (c->capturing) mg::fatal("%s is not possible while a CUDA graph is being captured (run one un-captured step first so that "
                                 "every buffer has its size)", what);
@@ -146,6 +184,8 @@ Ctx *create(int device, std::string *err) {
     Ctx *c = new Ctx();
     c->device = device;
     c->sms = prop.multiProcessorCount;
+    c->smem_block = prop.sharedMemPerBlock;
+    c->smem_optin = prop.sharedMemPerBlockOptin;
     CUDA_CHECK(cudaStreamCreate(&c->stream));
     CUDA_CHECK(cudaStreamCreateWithFlags(&c->copy, cudaStreamNonBlocking));
     CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_wire, cudaEventDisableTiming));
@@ -849,13 +889,14 @@ __global__ void __launch_bounds__(MASK_THREADS) random_legal_actions_kernel(cons
 }
 
 static int mask_chunks_per_arena(const EngineDev &hE, int group) { return (hE.grp[group].cap + MASK_THREADS - 1) / MASK_THREADS; }
+// dynamic shared memory of both mask kernels: MASK_THREADS rows and the 16 bytes of the store's alignment shift
+static size_t mask_dyn_smem(const EngineDev &hE, int group) { return (size_t)MASK_THREADS * hE.grp[group].n_action + 16; }
 
 void launch_action_mask(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group, unsigned char *out,
                         int n_total) {
     DeviceGuard guard(c);
-    const int na = hE.grp[group].n_action;
-    const size_t smem = (size_t)MASK_THREADS * na + 16;
-    if (smem + sizeof(EngineDev) > 48 * 1024) mg::fatal("action mask: %d actions per agent are more than the kernels hold", na);
+    const size_t smem = mask_dyn_smem(hE, group);
+    smem_prepare(c, ATTR_MASK, action_mask_kernel, smem, "action_mask_kernel");
     const int cpa = mask_chunks_per_arena(hE, group);
     action_mask_kernel<<<(unsigned)((size_t)hE.A * cpa), MASK_THREADS, smem, c->stream>>>(dE, curmask, group, out, n_total, cpa);
     post_launch("action_mask_kernel");
@@ -1007,14 +1048,17 @@ __global__ void __launch_bounds__(MEAN_THREADS, 5) mean_action_kernel(const Engi
     mean_action_cta<false>(E, curmask, g, of, mean, count, a, c0, cta_cnt, o0, nullptr, o0, mean_smem, n_in_s);
 }
 
+// dynamic shared memory of both mean-action kernels: the view LUT (one per heading in turn_mode) and the warps' histograms
+static size_t mean_dyn_smem(const EngineDev &hE, int group, int of) {
+    return (size_t)(hE.turn_mode ? 4 : 1) * hE.grp[group].view_count * sizeof(int2) +
+           (size_t)MEAN_WARPS * hE.grp[of].n_action * sizeof(int);
+}
+
 void launch_mean_action(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curmask, int group, int of,
                         float *mean, int *count, int n_total) {
     DeviceGuard guard(c);
-    const size_t smem = (size_t)(hE.turn_mode ? 4 : 1) * hE.grp[group].view_count * sizeof(int2) +
-                        (size_t)MEAN_WARPS * hE.grp[of].n_action * sizeof(int);
-    if (smem + sizeof(EngineDev) + 64 > 227 * 1024)
-        mg::fatal("mean action: a view of %d cells is more than the kernel holds", hE.grp[group].view_count);
-    if (smem + sizeof(EngineDev) + 64 > 48 * 1024) ensure_dynamic_smem(c->device, ATTR_MEAN, mean_action_kernel, smem);
+    const size_t smem = mean_dyn_smem(hE, group, of);
+    smem_prepare(c, ATTR_MEAN, mean_action_kernel, smem, "mean_action_kernel");
     const int cpa = (hE.grp[group].cap + MEAN_OBS - 1) / MEAN_OBS;
     mean_action_kernel<<<(unsigned)((size_t)hE.A * cpa), MEAN_THREADS, smem, c->stream>>>(dE, curmask, group, of, mean,
                                                                                           count, n_total, cpa);
@@ -1232,7 +1276,7 @@ void launch_obs_prepare(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsign
         CUDA_CHECK(cudaMemsetAsync(c->mm_pad, 0, need * sizeof(float), c->stream));
         c->mm_pad_n = need;
     }
-    if (cap_max <= 8192 && (size_t)cells * sizeof(int) <= 48 * 1024) {
+    if (cap_max <= 8192 && smem_band(c, ATTR_MINIMAP_SMALL, minimap_small_kernel, (size_t)cells * sizeof(int)) == 0) {
         minimap_small_kernel<<<hE.A * hE.G, 256, cells * sizeof(int), c->stream>>>(dE, curmask, og, c->mm_pad, c->mm_stride);
         post_launch("minimap_small_kernel");
         return;
@@ -1811,7 +1855,7 @@ obs_render_kernel(const __grid_constant__ ObsParams P) {
 // CTAs per SM of one render instantiation at this shared-memory size (0: it does not fit), cached per context slot
 template <typename T, int NIT, bool TURN, int TA>
 static int obs_ctas_per_sm(Ctx *c, int cfg_slot, size_t smem) {
-    if (smem > 227 * 1024) return 0;
+    if (smem_band(c, ATTR_OBS0 + cfg_slot, obs_render_kernel<T, NIT, TURN, TA>, smem) < 0) return 0;
     Ctx::ObsCfg &cfg = c->obs_cfg[cfg_slot];
     ensure_dynamic_smem(c->device, ATTR_OBS0 + cfg_slot, obs_render_kernel<T, NIT, TURN, TA>, smem);
     if (smem != cfg.smem) {
@@ -1897,7 +1941,10 @@ static void launch_obs_typed(Ctx *c, int cfg_slot, const EngineDev &hE, const Ob
     constexpr int TN = obs_tile_narrow<T>(), TW = obs_tile_wide<T>();
     const size_t lut_bytes = (size_t)(P.turn ? 4 : 1) * ((P.cells + 1) & ~1) * sizeof(int2);
     const size_t smem_n = (size_t)TN * P.rec * sizeof(T) + lut_bytes, smem_w = (size_t)TW * P.rec * sizeof(T) + lut_bytes;
-    if (smem_n > 227 * 1024) mg::fatal("observation record too large for the render kernel (%zu bytes of shared memory)", smem_n);
+    size_t need_n;
+    if (smem_band(c, ATTR_OBS0 + 2 * cfg_slot, obs_render_kernel<T, NIT, TURN, TN>, smem_n, &need_n) < 0)
+        mg::fatal("observation record too large for the render kernel (%zu bytes of shared memory, more than the %zu one "
+                  "block may use)", need_n, c->smem_optin);
     const int ctas_w = obs_ctas_per_sm<T, NIT, TURN, TW>(c, 2 * cfg_slot + 1, smem_w);
     const int ctas_n = obs_ctas_per_sm<T, NIT, TURN, TN>(c, 2 * cfg_slot, smem_n);
     const bool wide = O.tile == 0 ? ctas_w >= 1 && ctas_w * TW >= ctas_n * TN : O.tile == 2 && ctas_w >= 1;
@@ -2415,6 +2462,13 @@ __global__ void __launch_bounds__(256) obs_wire_kernel(const __grid_constant__ O
     }
 }
 
+// dynamic shared memory of obs_wire_kernel: the view LUT of the group, one per heading in turn_mode.  The kernel does not
+// opt in to more than the default per-block limit: a larger view takes the dense path (smem_fits SMEM_OBS_WIRE).
+static size_t wire_dyn_smem(const EngineDev &hE, int group) {
+    const GroupDev &G = hE.grp[group];
+    return (size_t)(hE.turn_mode ? 4 : 1) * ((G.view_w * G.view_h + 1) & ~1) * sizeof(int2);
+}
+
 __global__ void __launch_bounds__(1024) wire_scan_kernel(const int *chunk_total, long long *base, int n_chunks) {
     __shared__ long long carry_s;
     if (threadIdx.x == 0) carry_s = 0;
@@ -2497,8 +2551,9 @@ void obs_wire_begin(Ctx *c, const EngineDev *, const EngineDev &hE, const ObsArg
     }
     CUDA_CHECK(cudaMemsetAsync(c->wire_chunk_total, 0, (size_t)n_chunks * sizeof(int), c->stream));
     {
-        const size_t smem = (size_t)(P.turn ? 4 : 1) * ((P.cells + 1) & ~1) * sizeof(int2);
-        if (smem > 48 * 1024) mg::fatal("view too large for the wire kernel (%zu bytes of shared memory)", smem);
+        const size_t smem = wire_dyn_smem(hE, O.group);
+        if (smem_band(c, ATTR_WIRE, obs_wire_kernel, smem) != 0)
+            mg::fatal("view too large for the wire kernel (%zu bytes of shared memory)", smem);
         int grid = (n_total + 7) / 8;
         if (grid > 8 * c->sms) grid = 8 * c->sms;
         obs_wire_kernel<<<grid, 256, smem, c->stream>>>(P, c->wire_hdr, c->wire_slots, n_in, c->wire_chunk_total);
@@ -2756,9 +2811,8 @@ void launch_action_mask_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, 
     DeviceGuard guard(c);
     const size_t n = (size_t)hE.A * S;
     if (n == 0) return;
-    const int na = hE.grp[group].n_action;
-    const size_t smem = (size_t)MASK_THREADS * na + 16;
-    if (smem + sizeof(EngineDev) > 48 * 1024) mg::fatal("action mask: %d actions per agent are more than the kernels hold", na);
+    const size_t smem = mask_dyn_smem(hE, group);
+    smem_prepare(c, ATTR_MASK_SLOTS, action_mask_slots_kernel, smem, "action_mask_slots_kernel");
     slot_rows_scratch(c, hE, T, curmask, group, S, "growing the slot table of the slot-ordered action mask");
     const int cps = (S + MASK_THREADS - 1) / MASK_THREADS;
     action_mask_slots_kernel<<<(unsigned)((size_t)hE.A * cps), MASK_THREADS, smem, c->stream>>>(dE, curmask, group,
@@ -2807,12 +2861,8 @@ void launch_mean_action_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, 
     const size_t n = (size_t)hE.A * S;
     if (n == 0) return;
     if (n > 0x7fffffff) mg::fatal("%zu slots are more than one launch covers (rows a * S + slot are ints)", n);
-    const size_t smem = (size_t)(hE.turn_mode ? 4 : 1) * hE.grp[group].view_count * sizeof(int2) +
-                        (size_t)MEAN_WARPS * hE.grp[of].n_action * sizeof(int);
-    if (smem + sizeof(EngineDev) + 64 > 227 * 1024)
-        mg::fatal("mean action: a view of %d cells is more than the kernel holds", hE.grp[group].view_count);
-    if (smem + sizeof(EngineDev) + 64 > 48 * 1024)
-        ensure_dynamic_smem(c->device, ATTR_MEAN_SLOTS, mean_action_slots_kernel, smem);
+    const size_t smem = mean_dyn_smem(hE, group, of);
+    smem_prepare(c, ATTR_MEAN_SLOTS, mean_action_slots_kernel, smem, "mean_action_slots_kernel");
     slot_rows_scratch(c, hE, T, curmask, group, S, "growing the slot table of the slot-ordered mean action");
     const int cps = (S + MEAN_OBS - 1) / MEAN_OBS;
     mean_action_slots_kernel<<<(unsigned)((size_t)hE.A * cps), MEAN_THREADS, smem, c->stream>>>(
@@ -2832,6 +2882,35 @@ void launch_neighbours_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, c
     neighbours_slots_kernel<<<(unsigned)((size_t)hE.A * cps), NBR_THREADS, 0, c->stream>>>(
         dE, lut, curmask, group, of, k, c->obs_slot_row, S, T, S_of, idx, rel, count, cps);
     post_launch("neighbours_slots_kernel");
+}
+
+bool smem_fits(Ctx *c, const EngineDev &hE, int which, int group, int of, std::string *why) {
+    DeviceGuard guard(c);
+    size_t dyn = 0, need = 0;
+    int band = 0;
+    switch (which) {
+    case SMEM_ACTION_MASK:
+        band = smem_band(c, ATTR_MASK, action_mask_kernel, dyn = mask_dyn_smem(hE, group), &need); break;
+    case SMEM_ACTION_MASK_SLOTS:
+        band = smem_band(c, ATTR_MASK_SLOTS, action_mask_slots_kernel, dyn = mask_dyn_smem(hE, group), &need); break;
+    case SMEM_MEAN_ACTION:
+        band = smem_band(c, ATTR_MEAN, mean_action_kernel, dyn = mean_dyn_smem(hE, group, of), &need); break;
+    case SMEM_MEAN_ACTION_SLOTS:
+        band = smem_band(c, ATTR_MEAN_SLOTS, mean_action_slots_kernel, dyn = mean_dyn_smem(hE, group, of), &need); break;
+    case SMEM_OBS_WIRE:                                      // no opt-in: the default limit is the wire kernel's
+        band = smem_band(c, ATTR_WIRE, obs_wire_kernel, dyn = wire_dyn_smem(hE, group), &need);
+        if (band > 0) band = -1;
+        break;
+    default: mg::fatal("smem_fits: no kernel %d", which);
+    }
+    if (band >= 0) return true;
+    if (why) {
+        char buf[256];
+        snprintf(buf, sizeof buf, "%zu bytes of shared memory per block (%zu of them the kernel's own), more than the %zu "
+                 "the device allows", need, need - dyn, which == SMEM_OBS_WIRE ? c->smem_block : c->smem_optin);
+        *why = buf;
+    }
+    return false;
 }
 
 }  // namespace be

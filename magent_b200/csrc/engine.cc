@@ -52,6 +52,19 @@ static int refuse(const char *fmt, ...) {
     return -1;
 }
 
+// whether the kernel of a mask or mean-action call fits the device's shared memory (be::smem_fits); the refusal names
+// the call, the group's view or action space and the bytes.  Asked after to_device, before anything is staged or written.
+static bool smem_refused(be::Ctx *bx, const EngineDev &hE, int which, int group, int of, const char *call) {
+    std::string why;
+    if (!be::smem_fits || be::smem_fits(bx, hE, which, group, of, &why)) return false;
+    if (which == be::SMEM_ACTION_MASK || which == be::SMEM_ACTION_MASK_SLOTS)
+        refuse("%s: the %d actions of group %d need %s", call, hE.grp[group].n_action, group, why.c_str());
+    else
+        refuse("%s: a view of %d cells of group %d and the %d actions of group %d need %s", call, hE.grp[group].view_count,
+               group, hE.grp[of].n_action, of, why.c_str());
+    return true;
+}
+
 // ---------------------------------------------------------------------------------------------
 // ranges  (reference src/gridworld/Range.h:149-190; same double-precision arithmetic)
 RangeTab make_circle_range(float radius, float inner_radius, int parity) {
@@ -1104,9 +1117,11 @@ void Engine::get_observation(int group, void **bufs, int half) {      // GridWor
         host_path_ = (e && !strcmp(e, "dense")) ? 0 : (e && !strcmp(e, "wire")) ? 2 : 1;
     }
     // small observations (a few MB) are latency-, not bandwidth-bound: one plain copy of the dense records beats the
-    // wire protocol's fixed costs (totals read-back, waves, waking the pool)
+    // wire protocol's fixed costs (totals read-back, waves, waking the pool).  A view whose LUT the wire kernel cannot
+    // hold takes the dense path whatever the setting.
     if (!vdev && !fdev && !half && (host_path_ == 2 || (host_path_ == 1 && vbytes >= ((size_t)16 << 20))) && t.view.height * t.view.width < 0xffff &&
-        (long long)t.view.height * t.view.width * n_channel() < (1ll << 30)) {
+        (long long)t.view.height * t.view.width * n_channel() < (1ll << 30) &&
+        (!be::smem_fits || be::smem_fits(bx_, hE_, be::SMEM_OBS_WIRE, group, group, nullptr))) {
         get_observation_wire(group, bufs);
         return;
     }
@@ -1394,6 +1409,7 @@ int Engine::get_action_mask(int group, unsigned char *buf) {
     if (group < 0 || group >= G()) return refuse("invalid group handle %d in get_action_mask", group);
     if (!be::launch_action_mask) return refuse("the %s backend has no action-mask kernel", be::name());
     to_device();
+    if (smem_refused(bx_, hE_, be::SMEM_ACTION_MASK, group, group, "get_action_mask")) return -1;
     const bool dev = be::is_device_ptr(buf);
     if (!dev) settle_counts();
     const int n = total(group);
@@ -1424,6 +1440,7 @@ int Engine::get_mean_action(int group, int of, float *mean, int *count) {
     if (mem < 0) return -1;
     const bool dev = mean && mem;       // a null mean counts as host memory (refused below unless the group is empty)
     to_device();
+    if (smem_refused(bx_, hE_, be::SMEM_MEAN_ACTION, group, of, "get_mean_action")) return -1;
     if (!dev) settle_counts();
     const int n = total(group);
     if (n == 0) return 0;
@@ -1558,6 +1575,7 @@ int Engine::get_action_mask_slots(int group, unsigned char *mask) {
         return refuse("the %s backend has no slot-ordered action-mask kernel", be::name());
     const int mem = out_memory("get_action_mask_slots: mask", {mask});
     to_device();
+    if (smem_refused(bx_, hE_, be::SMEM_ACTION_MASK_SLOTS, group, group, "get_action_mask_slots")) return -1;
     const int S = slot_space(group);
     read_back(mem == 1, {{mask, (size_t)A_ * S * group_type_[group]->n_action}}, [&](void **to) {
         be::launch_action_mask_slots(bx_, dE_, hE_, d_slot_dev_, curmask_, group, S, (unsigned char *)to[0]);
@@ -1575,6 +1593,7 @@ int Engine::get_mean_action_slots(int group, int of, float *mean, int *count) {
     const int mem = out_memory("get_mean_action_slots: mean and count", {mean, count});
     if (mem < 0) return -1;
     to_device();
+    if (smem_refused(bx_, hE_, be::SMEM_MEAN_ACTION_SLOTS, group, of, "get_mean_action_slots")) return -1;
     const int S = slot_space(group);
     const size_t n = (size_t)A_ * S;
     read_back(mem == 1, {{mean, n * group_type_[of]->n_action * 4}, {count, n * 4}}, [&](void **to) {
