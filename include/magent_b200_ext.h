@@ -188,6 +188,47 @@ int magent_b200_get_action_mask_slots(EnvHandle game, GroupHandle group, unsigne
 int magent_b200_get_mean_action_slots(EnvHandle game, GroupHandle group, GroupHandle of, float *mean, int *count);
 int magent_b200_get_neighbours_slots(EnvHandle game, GroupHandle group, GroupHandle of, int k, int *idx, int *rel,
                                      int *count);
+/* Built-in scripted opponents: a fixed, non-trivial policy to train against or to measure progress by, decided on the
+ * device.  For every agent i of `group` and a target group `target` (t; t == group allowed), on the state as it is now:
+ *   MAGENT_B200_RULE_RUSH
+ *     1. attack: among the attack actions k that magent_b200_get_action_mask allows i and whose aimed cell holds an agent
+ *        of t other than i, the one whose target agent has the lowest hp now (env_get_info "hp"); ties to the lowest k.
+ *     2. approach: otherwise, when i sees an agent of t, let c be the map cell that magent_b200_get_neighbours(group,
+ *        of = t, k = 1) lists for i (its nearest visible target, at its smallest-key cell; turn_mode headings, sector
+ *        views and longer bodies as stated there).  Among the move actions k < n_move that the mask allows (turn actions
+ *        never count), the one whose moved footprint [nx, nx + bw) x [ny, ny + bh) (the body after the move, rotated by
+ *        i's heading) has the smallest squared distance to c: ex^2 + ey^2, ex = nx - cx when cx < nx, cx - (nx + bw - 1)
+ *        when cx >= nx + bw, else 0 (ey likewise), as the neighbours' key measures d2.  Ties to the lowest k.
+ *     3. fallback: otherwise, the action magent_b200_random_legal_actions(game, group, seed) would set for i if it were
+ *        called in this call's place.  This call does not count as one of its calls: it leaves the call counter that
+ *        random_actions and random_legal_actions share where it was.
+ *   MAGENT_B200_RULE_FLEE: step 2 with the largest distance instead of the smallest, when i sees an agent of t; otherwise
+ *     step 3.
+ * Step 2 with no legal move falls through to step 3.  A dead, un-culled agent and an agent with no legal action take
+ * action 0, which the step ignores for it.  Food cells (food_mode) are never targets; an absorber is one like any agent.
+ * Typical targets: the enemy in battle, the prey for pursuit's predators (rush), the predators for pursuit's prey (flee),
+ * the food group in gather.  The fallback, like random_legal_actions, folds the device step counter into the seed, so
+ * a replayed CUDA graph draws afresh.
+ *   rule_actions: sets the decisions as the group's actions for this step; it counts as the group's set_action (same
+ *     place in the step's action order, blocks magent_b200_restore_arenas until env_step).  No synchronisation and no
+ *     allocation: recordable into a CUDA graph.
+ *   get_rule_actions: int32 [n] in row order (the rows of env_set_action), the actions rule_actions would set.  Host
+ *     pointer: the call waits for the counts.  CUDA device pointer: no synchronisation, no allocation, recordable into a
+ *     CUDA graph; rows are sized by the device-side counts, at most "num_bound" of them are written.
+ *   get_rule_actions_slots: int32 [A][S] in the [arena, slot] layout of magent_b200_get_slots: an occupied slot holds the
+ *     row call's action for row slot_row[a][s], a vacant slot -1.  Does not wait for the counts, whatever the pointer
+ *     kind; CUDA device pointer: no synchronisation and, once a first call has sized the engine's tables, no allocation.
+ * None of them sets or reads anything else.  They cover every arena whatever magent_b200_select_arena says.  Returns -1,
+ * sets magent_b200_last_error and writes or registers nothing for a bad `group` or `target` handle, a policy other than
+ * the two below, a NULL act where something is to be written, a view of `group` too large to order its cells by an int key
+ * (as magent_b200_get_neighbours refuses it), or a backend without the kernel. */
+#define MAGENT_B200_RULE_RUSH 0
+#define MAGENT_B200_RULE_FLEE 1
+int magent_b200_rule_actions(EnvHandle game, GroupHandle group, GroupHandle target, int policy, unsigned long long seed);
+int magent_b200_get_rule_actions(EnvHandle game, GroupHandle group, GroupHandle target, int policy,
+                                 unsigned long long seed, int *act);
+int magent_b200_get_rule_actions_slots(EnvHandle game, GroupHandle group, GroupHandle target, int policy,
+                                       unsigned long long seed, int *act);
 /* compact observation hand-off (SURVEY.md 8f rank 2): same call, layout and pointer rules as env_get_observation
  * (reference src/runtime_api.h:35), but every element is an IEEE binary16 = the float32 value rounded to
  * nearest-even.  buffer[0] = view [n][view_h][view_w][n_channel], buffer[1] = feature [n][feature_size];

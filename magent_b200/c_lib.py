@@ -74,6 +74,10 @@ EXT_SIGNATURES = {
     "magent_b200_get_action_mask_slots": ([_vp, ctypes.c_int, _vp], ctypes.c_int),
     "magent_b200_get_mean_action_slots": ([_vp, ctypes.c_int, ctypes.c_int, _vp, _vp], ctypes.c_int),
     "magent_b200_get_neighbours_slots": ([_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp], ctypes.c_int),
+    "magent_b200_rule_actions": ([_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_ulonglong], ctypes.c_int),
+    "magent_b200_get_rule_actions": ([_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_ulonglong, _vp], ctypes.c_int),
+    "magent_b200_get_rule_actions_slots": ([_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_ulonglong, _vp],
+                                           ctypes.c_int),
     "magent_b200_get_observation_f16": ([_vp, ctypes.c_int, ctypes.POINTER(_vp)], ctypes.c_int),
     "magent_b200_get_global_state": ([_vp, _vp, ctypes.c_int], ctypes.c_int),
     "magent_b200_snapshot_arenas": ([_vp], ctypes.c_int),

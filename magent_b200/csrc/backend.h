@@ -139,6 +139,19 @@ __attribute__((weak)) void launch_mean_action_slots(Ctx *, const EngineDev *dE, 
 __attribute__((weak)) void launch_neighbours_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
                                                    const NbrCell *lut, unsigned curmask, int group, int of, int k, int S,
                                                    int S_of, int *idx, int *rel, int *count);
+// The built-in scripted opponent (rule_phases.h rule_action) for every agent of `group` against group `target` under
+// `policy` (RULE_RUSH, RULE_FLEE); `seed` and the device step counter as legal_draw takes them, `lut` as for
+// launch_neighbours.  launch_rule_actions: int [n] in row order into `out`, or AgentSoA::act of every agent when `out` is
+// null; n_total is the host's count, an upper bound: the device-side offsets decide.  launch_rule_actions_slots: int
+// [A][S] into `out`, the action of the row in each slot (slot_phases.h, the device-side offsets decide the rows), -1
+// where no row is.  All buffers are device buffers.  Weak like launch_neighbours: the engine refuses the calls without
+// them.
+__attribute__((weak)) void launch_rule_actions(Ctx *, const EngineDev *dE, const EngineDev &hE, const NbrCell *lut,
+                                               unsigned curmask, int group, int target, int policy,
+                                               unsigned long long seed, int *out, int n_total);
+__attribute__((weak)) void launch_rule_actions_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
+                                                     const NbrCell *lut, unsigned curmask, int group, int target,
+                                                     int policy, unsigned long long seed, int S, int *out);
 // Whether kernel `which` fits the device's shared memory for `group` (and, for the mean action, the histograms of group
 // `of`'s actions): its static shared memory plus what the view or the action space asks for, against the device's
 // opt-in limit per block (the default limit for the wire kernel, which does not opt in).  When it does not, *why (unless

@@ -29,6 +29,7 @@ namespace mg { __device__ long long mg_phase_clock[8 * 32]; }
 #include "obs_phases.h"
 #include "mask_phases.h"
 #include "nbr_phases.h"
+#include "rule_phases.h"
 #include "slot_phases.h"
 
 namespace cg = cooperative_groups;
@@ -2882,6 +2883,127 @@ void launch_neighbours_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, c
     neighbours_slots_kernel<<<(unsigned)((size_t)hE.A * cps), NBR_THREADS, 0, c->stream>>>(
         dE, lut, curmask, group, of, k, c->obs_slot_row, S, T, S_of, idx, rel, count, cps);
     post_launch("neighbours_slots_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
+// built-in scripted opponents (magent_b200_rule_actions, _get_rule_actions, _get_rule_actions_slots): rule_phases.h
+// for every agent of a group.  CTAs are dealt per arena like random_legal_actions_kernel (blockIdx says which arena, the
+// device-side offsets decide how many agents it has, the host's count is only an upper bound); a thread holds one agent.
+// Attacks, moves and the fallback draw are decided per lane (rule_attack, rule_move, rule_fallback: a handful of `occ`
+// cells each).  The view walk of step 2 (rule_nearest) is made by the whole warp, one agent at a time for the lanes
+// that need it: the lanes take 32 consecutive cells of the view LUT (key order, L1-resident), and the lowest lane whose
+// cell lists a target in the first round that has one gives the cell, as neighbours_kernel finds its first neighbour.
+// A walk of one lane at a time measured about 1.24 ms per call on battle512 against 0.19 ms for the neighbours at k = 1
+// (DESIGN.md §5).  The slot kernel takes RULE_THREADS consecutive slots of one arena per CTA and looks each slot's row up
+// in slots_kernel's [A][S] map, as action_mask_slots_kernel does; a vacant slot gets -1.
+constexpr int RULE_THREADS = 256;
+// __launch_bounds__(RULE_THREADS, 4) leaves them 64 registers: 61-63 without spills (a bare bound allows 48, and spills).
+
+// The action of this lane's agent m (ABI ordinal o; `live` false: no agent, the result is not used).  Every lane of the
+// warp calls it.
+__device__ __forceinline__ int rule_warp(const EngineDev &E, const NbrCell *lut, unsigned curmask, int a, int g, int t,
+                                         int policy, const MaskAgent &m, bool live, unsigned long long seed, int o) {
+    const int lane = threadIdx.x & 31;
+    const int *occ = E.occ + (long)a * E.W * E.H;
+    int act = -1;                                             // -1: not decided yet
+    if (!live || (m.flags & FLAG_DEAD)) act = 0;
+    else if (policy == RULE_RUSH) act = rule_attack(E, curmask, a, occ, g, t, m);
+    const int n = E.grp[g].view_count;
+    bool seen = false;
+    int cx = 0, cy = 0;
+    for (unsigned need = __ballot_sync(0xffffffffu, act < 0); need; need &= need - 1) {
+        const int u = __ffs(need) - 1;
+        NbrObserver w;
+        w.x = __shfl_sync(0xffffffffu, m.x, u); w.y = __shfl_sync(0xffffffffu, m.y, u);
+        w.dir = __shfl_sync(0xffffffffu, m.dir, u); w.code = __shfl_sync(0xffffffffu, m.code, u);
+        w.flags = (unsigned char)__shfl_sync(0xffffffffu, (int)m.flags, u);
+        const NbrCell *l = lut + (E.turn_mode ? w.dir * n : 0);
+        const unsigned char *kp = E.kind + (long)a * E.kplane + (long)(w.y + E.kpad) * E.kw + w.x + E.kpad;
+        for (int q0 = 0; q0 < n; q0 += 32) {                  // warp-uniform bounds: every lane takes every ballot
+            const int q = q0 + lane;
+            int x = 0, y = 0;
+            bool hit = false;
+            if (q < n && nbr_kind_of(__ldg(kp + __ldg(&l[q].off)), t)) {
+                const int d = __ldg(&l[q].delta);
+                x = w.x + (short)(d & 0xffff); y = w.y + (d >> 16);
+                hit = nbr_nearest_at(E, curmask, a, g, t, w, x, y, __ldg(&l[q].key)) >= 0;
+            }
+            const unsigned hits = __ballot_sync(0xffffffffu, hit);
+            if (hits) {
+                const int f = __ffs(hits) - 1;
+                x = __shfl_sync(0xffffffffu, x, f); y = __shfl_sync(0xffffffffu, y, f);
+                if (lane == u) { seen = true; cx = x; cy = y; }
+                break;
+            }
+        }
+    }
+    if (act < 0 && seen) act = rule_move(E, curmask, a, occ, g, m, cx, cy, policy == RULE_FLEE);
+    if (act < 0) act = rule_fallback(E, curmask, a, occ, g, m, seed, E.counters[CNT_STEPS], o);
+    return act;
+}
+
+__global__ void __launch_bounds__(RULE_THREADS, 4) rule_actions_kernel(const EngineDev *gE, const NbrCell *lut,
+                                                                      unsigned curmask, int g, int t, int policy,
+                                                                      unsigned long long seed, int *out, int n_total,
+                                                                      int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int *off = E.off + (size_t)g * (E.A + 1);
+    const int a = blockIdx.x / chunks_per_arena;
+    const int c0 = (blockIdx.x - a * chunks_per_arena) * RULE_THREADS;
+    const int o0 = off[a];
+    if (c0 >= off[a + 1] - o0 || o0 + c0 >= n_total) return;     // the whole CTA: the warps below stay converged
+    const int i = c0 + threadIdx.x, o = o0 + i;
+    const bool live = i < off[a + 1] - o0 && o < n_total;
+    MaskAgent m;
+    m.x = m.y = 0; m.dir = DIR_NORTH; m.code = 0; m.flags = FLAG_DEAD;
+    if (live) m = mask_agent(E, curmask, a, g, i);
+    const int act = rule_warp(E, lut, curmask, a, g, t, policy, m, live, seed, o);
+    if (!live) return;
+    if (out) out[o] = act;
+    else cur_soa(E, curmask, g).act[gidx(E, a, g, i)] = act;
+}
+
+__global__ void __launch_bounds__(RULE_THREADS, 4) rule_actions_slots_kernel(const EngineDev *gE, const NbrCell *lut,
+                                                                            unsigned curmask, int g, int t, int policy,
+                                                                            unsigned long long seed, const int *slot_row,
+                                                                            int S, int *out, int chunks_per_arena) {
+    __shared__ EngineDev sE;
+    load_engine(&sE, gE);
+    const EngineDev &E = sE;
+    const int a = blockIdx.x / chunks_per_arena;
+    const int s = (blockIdx.x - a * chunks_per_arena) * RULE_THREADS + threadIdx.x;
+    const int r = s < S ? slot_row[(long)a * S + s] : -1;
+    const int o0 = E.off[(size_t)g * (E.A + 1) + a];
+    MaskAgent m;
+    m.x = m.y = 0; m.dir = DIR_NORTH; m.code = 0; m.flags = FLAG_DEAD;
+    if (r >= 0) m = mask_agent(E, curmask, a, g, r - o0);
+    const int act = rule_warp(E, lut, curmask, a, g, t, policy, m, r >= 0, seed, r);
+    if (s < S) out[(long)a * S + s] = r >= 0 ? act : -1;
+}
+
+void launch_rule_actions(Ctx *c, const EngineDev *dE, const EngineDev &hE, const NbrCell *lut, unsigned curmask,
+                         int group, int target, int policy, unsigned long long seed, int *out, int n_total) {
+    DeviceGuard guard(c);
+    const int cpa = (hE.grp[group].cap + RULE_THREADS - 1) / RULE_THREADS;
+    rule_actions_kernel<<<(unsigned)((size_t)hE.A * cpa), RULE_THREADS, 0, c->stream>>>(dE, lut, curmask, group, target,
+                                                                                      policy, seed, out, n_total, cpa);
+    post_launch("rule_actions_kernel");
+}
+
+void launch_rule_actions_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE, const SlotDev *T, const NbrCell *lut,
+                               unsigned curmask, int group, int target, int policy, unsigned long long seed, int S,
+                               int *out) {
+    DeviceGuard guard(c);
+    const size_t n = (size_t)hE.A * S;
+    if (n == 0) return;
+    if (n > 0x7fffffff) mg::fatal("%zu slots are more than one launch covers (rows a * S + slot are ints)", n);
+    slot_rows_scratch(c, hE, T, curmask, group, S, "growing the slot table of the slot-ordered rule actions");
+    const int cps = (S + RULE_THREADS - 1) / RULE_THREADS;
+    rule_actions_slots_kernel<<<(unsigned)((size_t)hE.A * cps), RULE_THREADS, 0, c->stream>>>(
+        dE, lut, curmask, group, target, policy, seed, c->obs_slot_row, S, out, cps);
+    post_launch("rule_actions_slots_kernel");
 }
 
 bool smem_fits(Ctx *c, const EngineDev &hE, int which, int group, int of, std::string *why) {

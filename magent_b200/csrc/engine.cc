@@ -2,6 +2,7 @@
 #include "engine.h"
 #include "step_phases.h"
 #include "nbr_phases.h"
+#include "rule_phases.h"
 #include "slot_phases.h"
 
 #include <math.h>
@@ -1621,6 +1622,56 @@ int Engine::get_neighbours_slots(int group, int of, int k, int *idx, int *rel, i
     read_back(mem == 1, {{idx, idx_bytes}, {rel, 2 * idx_bytes}, {count, n * 4}}, [&](void **to) {
         be::launch_neighbours_slots(bx_, dE_, hE_, d_slot_dev_, d_nbr_lut_ + nbr_lut_base_[group], curmask_, group, of,
                                     k, S, slot_space(of), (int *)to[0], (int *)to[1], (int *)to[2]);
+    });
+    return 0;
+}
+
+// The built-in scripted opponent.  The fallback draws as random_legal_actions would if it were called next: the seed it
+// would see, without counting as one of its calls, so that the three variants agree and leave the draws of
+// random_actions / random_legal_actions as they were.
+bool Engine::rule_refused(int group, int target, int policy, bool slots, const char *what) {
+    if (group < 0 || group >= G()) return refuse("invalid group handle %d in %s", group, what) < 0;
+    if (target < 0 || target >= G()) return refuse("invalid group handle %d for `target` in %s", target, what) < 0;
+    if (policy != RULE_RUSH && policy != RULE_FLEE)
+        return refuse("%s: policy %d is neither rush (%d) nor flee (%d)", what, policy, RULE_RUSH, RULE_FLEE) < 0;
+    if (slots ? !be::launch_rule_actions_slots || !be::launch_restore_slots : !be::launch_rule_actions)
+        return refuse("the %s backend has no %srule-action kernel", be::name(), slots ? "slot-ordered " : "") < 0;
+    to_device();
+    if (!nbr_key_fits_[group])
+        return refuse("%s: the view of group %d is too large to order its cells by an int key", what, group) < 0;
+    return false;
+}
+
+int Engine::rule_actions(int group, int target, int policy, unsigned long long seed) {
+    if (rule_refused(group, target, policy, false, "rule_actions")) return -1;
+    if (std::find(order_.begin(), order_.end(), group) == order_.end()) order_.push_back(group);
+    const int n = total(group);
+    if (n == 0) return 0;
+    be::launch_rule_actions(bx_, dE_, hE_, d_nbr_lut_ + nbr_lut_base_[group], curmask_, group, target, policy,
+                            seed * 0x9E3779B97F4A7C15ull + rand_calls_ + 1, nullptr, n);
+    return 0;
+}
+
+int Engine::get_rule_actions(int group, int target, int policy, unsigned long long seed, int *act) {
+    if (rule_refused(group, target, policy, false, "get_rule_actions")) return -1;
+    const bool dev = be::is_device_ptr(act);
+    if (!dev) settle_counts();
+    const int n = total(group);
+    if (n > 0 && !act) return refuse("get_rule_actions needs an action buffer");
+    read_back(dev, {{act, (size_t)n * 4}}, [&](void **to) {
+        be::launch_rule_actions(bx_, dE_, hE_, d_nbr_lut_ + nbr_lut_base_[group], curmask_, group, target, policy,
+                                seed * 0x9E3779B97F4A7C15ull + rand_calls_ + 1, (int *)to[0], n);
+    });
+    return 0;
+}
+
+int Engine::get_rule_actions_slots(int group, int target, int policy, unsigned long long seed, int *act) {
+    if (rule_refused(group, target, policy, true, "get_rule_actions_slots")) return -1;
+    const int S = slot_space(group);
+    if (S > 0 && !act) return refuse("get_rule_actions_slots needs an action buffer");
+    read_back(be::is_device_ptr(act), {{act, (size_t)A_ * S * 4}}, [&](void **to) {
+        be::launch_rule_actions_slots(bx_, dE_, hE_, d_slot_dev_, d_nbr_lut_ + nbr_lut_base_[group], curmask_, group,
+                                      target, policy, seed * 0x9E3779B97F4A7C15ull + rand_calls_ + 1, S, (int *)to[0]);
     });
     return 0;
 }

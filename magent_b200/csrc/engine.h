@@ -159,6 +159,12 @@ public:
     // last error when refused.
     int get_mean_action_slots(int group, int of, float *mean, int *count);
     int get_neighbours_slots(int group, int of, int k, int *idx, int *rel, int *count);
+    // the built-in scripted opponent (rule_phases.h) of one group against group `target`: set as the group's actions
+    // (rule_actions), int [n] in row order (get_rule_actions) or int [A][S] in slot order (get_rule_actions_slots).  -1
+    // and the last error when refused.
+    int rule_actions(int group, int target, int policy, unsigned long long seed);
+    int get_rule_actions(int group, int target, int policy, unsigned long long seed, int *act);
+    int get_rule_actions_slots(int group, int target, int policy, unsigned long long seed, int *act);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads
@@ -222,6 +228,7 @@ private:
     std::vector<size_t> nbr_lut_base_;
     std::vector<unsigned char> nbr_key_fits_;
     void upload_nbr_luts(bool force);
+    bool rule_refused(int group, int target, int policy, bool slots, const char *what);
     // stable slots: the live table ([A][SLOT_HDR + slot_id_cap_], grow-only, outside dev_allocs_ so that a re-allocation
     // of the device image does not drop it), the SlotDev block naming it (allocated once, so captured graphs stay valid
     // when the table grows), and slot_space_[g] = S(g) as the last reset, add_agents, snapshot_arenas or free_snapshot

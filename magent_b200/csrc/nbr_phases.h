@@ -57,6 +57,13 @@ MG_HD bool nbr_in_view(const EngineDev &E, const GroupDev &G, int dir, int dx, i
 }
 
 // ---- the order of magent_b200_get_neighbours
+// The squared Euclidean distance from the map cell at displacement (dx, dy) from a footprint's top-left corner to that
+// footprint [0, bw) x [0, bh): 0 on the footprint.
+MG_HD int nbr_box_d2(int bw, int bh, int dx, int dy) {
+    const int ex = dx < 0 ? -dx : dx >= bw ? dx - bw + 1 : 0;
+    const int ey = dy < 0 ? -dy : dy >= bh ? dy - bh + 1 : 0;
+    return ex * ex + ey * ey;
+}
 // The key of view cell (vx, vy) of an observer of group G facing `dir`, whose map cell lies at displacement (dx, dy) from
 // the observer's stored top-left corner: first d2, the squared Euclidean distance from that cell to the observer's
 // footprint [0, bw) x [0, bh) (0 on the footprint), then the row-major view index.  Packed as d2 * view cells + index,
@@ -64,9 +71,7 @@ MG_HD bool nbr_in_view(const EngineDev &E, const GroupDev &G, int dir, int dx, i
 MG_HD int nbr_cell_key(const GroupDev &G, int dir, int dx, int dy, int vx, int vy) {
     int bw, bh;
     body_dims(G, dir, bw, bh);
-    const int ex = dx < 0 ? -dx : dx >= bw ? dx - bw + 1 : 0;
-    const int ey = dy < 0 ? -dy : dy >= bh ? dy - bh + 1 : 0;
-    return (ex * ex + ey * ey) * (G.view_w * G.view_h) + vy * G.view_w + vx;
+    return nbr_box_d2(bw, bh, dx, dy) * (G.view_w * G.view_h) + vy * G.view_w + vx;
 }
 // the key of map displacement (dx, dy), or -1 when it is not on an in-range cell of the window
 MG_HD int nbr_key(const EngineDev &E, const GroupDev &G, int dir, int dx, int dy) {

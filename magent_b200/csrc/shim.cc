@@ -136,6 +136,18 @@ MG_API int magent_b200_get_neighbours_slots(EnvHandle game, GroupHandle group, G
                                             int *count) {
     return E(game)->get_neighbours_slots(group, of, k, idx, rel, count);
 }
+MG_API int magent_b200_rule_actions(EnvHandle game, GroupHandle group, GroupHandle target, int policy,
+                                    unsigned long long seed) {
+    return E(game)->rule_actions(group, target, policy, seed);
+}
+MG_API int magent_b200_get_rule_actions(EnvHandle game, GroupHandle group, GroupHandle target, int policy,
+                                        unsigned long long seed, int *act) {
+    return E(game)->get_rule_actions(group, target, policy, seed, act);
+}
+MG_API int magent_b200_get_rule_actions_slots(EnvHandle game, GroupHandle group, GroupHandle target, int policy,
+                                              unsigned long long seed, int *act) {
+    return E(game)->get_rule_actions_slots(group, target, policy, seed, act);
+}
 MG_API int magent_b200_get_observation_f16(EnvHandle game, GroupHandle group, void **buffer) {
     E(game)->get_observation(group, buffer, 1);
     return 0;

@@ -984,6 +984,76 @@ class GridWorld(Environment):
                                                                    _dptr(count)), "get_neighbours_slots")
         return idx, rel, count
 
+    # ---- built-in scripted opponents (include/magent_b200_ext.h magent_b200_rule_actions has the definition)
+    RULE_POLICIES = {"rush": 0, "flee": 1}
+
+    def _rule_args(self, handle, target, policy, seed):
+        if isinstance(policy, str):
+            if policy not in self.RULE_POLICIES:
+                raise ValueError("policy must be one of %s, got %r" % (sorted(self.RULE_POLICIES), policy))
+            policy = self.RULE_POLICIES[policy]
+        return self.game, self._hv(handle), self._hv(target), int(policy), int(seed)
+
+    def set_rule_actions(self, handle, target, policy="rush", seed=0):
+        """set_action with the built-in scripted opponent's choice for every agent of the group, decided on the device
+        against group `target`: "rush" attacks the weakest target in reach, else steps towards the nearest visible one;
+        "flee" steps away from the nearest visible one; both fall back to the draw of set_random_legal_actions(handle,
+        seed).  Nothing waits for the device, and the call can be recorded into a CUDA graph (capture_graph)."""
+        self._check(self._lib.magent_b200_rule_actions(*self._rule_args(handle, target, policy, seed)),
+                    "rule_actions")
+
+    def get_rule_actions(self, handle, target, policy="rush", seed=0):
+        """int32 (n,): the actions set_rule_actions would set, in the order of set_action.  The array is a cached
+        receive buffer: valid until the next call."""
+        g = self._hv(handle)
+        buf = self._host_view((g, "rule"), (self.get_num(handle),), np.int32)
+        self._check(self._lib.magent_b200_get_rule_actions(*self._rule_args(handle, target, policy, seed),
+                                                           buf.ctypes.data if buf.size else None), "get_rule_actions")
+        return buf
+
+    def get_rule_actions_torch(self, handle, target, policy="rush", seed=0, out=None):
+        """the scripted actions (see get_rule_actions) written straight into a CUDA int32 tensor (n,).
+
+        out: a caller-owned contiguous CUDA int32 tensor (rows,) with at least get_num_bound(handle) rows; needed to
+        record the call into a CUDA graph (capture_graph), since the call then allocates nothing.  Returns its first
+        get_num(handle) entries."""
+        import torch
+        n = self.get_num(handle)
+        if out is None:
+            out = torch.empty((n,), dtype=torch.int32, device="cuda")
+        else:
+            _check_cuda_out(out, "out", (torch.int32,), rows=self.get_num_bound(handle))
+        if out.numel():
+            self._check(self._lib.magent_b200_get_rule_actions(*self._rule_args(handle, target, policy, seed),
+                                                               _dptr(out)), "get_rule_actions")
+        return out[:n]
+
+    def get_rule_actions_slots(self, handle, target, policy="rush", seed=0):
+        """int32 (num_arenas, S): the scripted actions (see get_rule_actions) in the stable slot layout (see get_slots);
+        -1 in vacant slots.  The array is a cached receive buffer: valid until the next call."""
+        g = self._hv(handle)
+        buf = self._host_view((g, "rule_slots"), self._slot_shape(handle), np.int32)
+        self._check(self._lib.magent_b200_get_rule_actions_slots(*self._rule_args(handle, target, policy, seed),
+                                                                 buf.ctypes.data if buf.size else None),
+                    "get_rule_actions_slots")
+        return buf
+
+    def get_rule_actions_slots_torch(self, handle, target, policy="rush", seed=0, out=None):
+        """the slot-ordered scripted actions (see get_rule_actions_slots) written straight into a CUDA int32 tensor
+        (num_arenas, S), without waiting for the device.
+
+        out: a caller-owned contiguous CUDA int32 tensor of that shape; needed to record the call into a CUDA graph
+        (capture_graph), since the call then allocates nothing once a first call has run."""
+        import torch
+        shape = self._slot_shape(handle)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.int32, device="cuda")
+        else:
+            _check_cuda_out(out, "out", (torch.int32,), shape=shape)
+        self._check(self._lib.magent_b200_get_rule_actions_slots(*self._rule_args(handle, target, policy, seed),
+                                                                 _dptr(out)), "get_rule_actions_slots")
+        return out
+
     def get_counters(self):
         """int64 event counters accumulated on the device since construction"""
         buf = (ctypes.c_longlong * 16)()
