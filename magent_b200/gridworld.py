@@ -55,6 +55,16 @@ def _check_cuda_out(t, what, dtypes, rows=None, tail=(), shape=None, align=1, op
             what, ", %d-byte aligned" % align if align > 1 else "", " or ".join(map(str, dtypes)), want))
 
 
+def _out_tuple(out, parts):
+    """a caller's `out` as one entry per output part (see GridWorld._outputs): the tensor itself for one part, else a
+    tuple of tensors in which None may stand for optional parts, not for all"""
+    if len(parts) == 1:
+        return (out,)
+    if not isinstance(out, (tuple, list)) or len(out) != len(parts) or all(t is None for t in out):
+        raise ValueError("out must be a (%s) tuple of CUDA tensors, not all None" % ", ".join(p[0] for p in parts))
+    return tuple(out)
+
+
 class _HostBlock:
     """A growable host buffer; page-locked when the engine offers an allocator."""
 
@@ -453,25 +463,25 @@ class GridWorld(Environment):
         (device pointers are detected by the engine; no PCIe traffic).
 
         dtype: torch.float32 (default, the reference layout) or torch.float16 (compact hand-off: every element
-        is the float32 value rounded to nearest-even; half the bytes)."""
+        is the float32 value rounded to nearest-even; half the bytes).
+        out: a caller-owned (view, feature) pair of contiguous CUDA tensors of one of those dtypes, (rows,) + view_space
+        and (rows,) + feature_space with at least get_num(handle) rows; returned whole."""
         import torch
         g = self._hv(handle)
         n = self.get_num(handle)
         if out is None:
-            dtype = torch.float32 if dtype is None else dtype
-            view = torch.empty((n,) + self.view_space[g], dtype=dtype, device="cuda")
-            feat = torch.empty((n,) + self.feature_space[g], dtype=dtype, device="cuda")
+            view, feat = (torch.empty((n,) + tail, dtype=getattr(torch, dtypes[0]), device="cuda")
+                          for _name, dtypes, tail, _opt in self._obs_parts(g, dtype))
         else:
-            view, feat = out
-            dtype = view.dtype
-            assert feat.dtype == dtype and view.is_contiguous() and feat.is_contiguous()
+            # at least get_num rows: the engine writes that many records through device pointers
+            view, feat = _out_tuple(out, self._obs_parts(g))
+            _check_cuda_out(view, "view", (torch.float32, torch.float16), rows=n, tail=self.view_space[g])
+            _check_cuda_out(feat, "feature", (view.dtype,), rows=n, tail=self.feature_space[g])
         bufs = (ctypes.c_void_p * 2)(view.data_ptr(), feat.data_ptr())
-        if dtype == torch.float16:
+        if view.dtype == torch.float16:
             self._lib.magent_b200_get_observation_f16(self.game, g, bufs)
-        elif dtype == torch.float32:
-            self._lib.env_get_observation(self.game, g, bufs)
         else:
-            raise ValueError("observation dtype must be torch.float32 or torch.float16")
+            self._lib.env_get_observation(self.game, g, bufs)
         return view, feat
 
     def get_observation_f16(self, handle):
@@ -576,15 +586,72 @@ class GridWorld(Environment):
         """uniform random actions generated on the device (throughput runs only)"""
         self._lib.magent_b200_random_actions(self.game, self._hv(handle), None, int(seed))
 
+    # ---- per-agent outputs, in rows (the order of set_action) or in the stable slot layout (see get_slots).  Whether a
+    # call reaches the engine with nothing to write (an empty group, S = 0) is each method's own: the engine checks the
+    # arguments of any call it gets (groups, k, policy, a kernel's limits), and refuses an empty tensor's NULL data for
+    # a part it needs.
+    # An output part: (name, its torch dtype names, the first also its numpy dtype and the one allocated, its per-record
+    # shape, whether a caller's out may give None for it: passed as NULL, returned as None).
+    _RULE_PARTS = (("act", ("int32",), (), False),)
+    _REWARD_PARTS = (("reward", ("float32",), (), True), ("status", ("uint8",), (), True))
+
+    def _mask_parts(self, g):
+        return (("mask", ("bool", "uint8"), (self.action_space[g][0],), False),)
+
+    def _mean_parts(self, of, slots=False):          # count may be None in the slot-ordered form only
+        return (("mean", ("float32",), (self.action_space[of][0],), False), ("count", ("int32",), (), slots))
+
+    @staticmethod
+    def _nbr_parts(k):                              # (k, checked, and the parts)
+        k = int(k)
+        if not 1 <= k <= 32:
+            raise ValueError("k must be in [1, 32], got %d" % k)
+        return k, (("idx", ("int32",), (k,), False), ("rel", ("int32",), (k, 2), True), ("count", ("int32",), (), True))
+
+    def _obs_parts(self, g, dtype=None):            # float32 or float16, or the one of them `dtype` names
+        if dtype is not None and str(dtype) not in ("torch.float32", "torch.float16"):
+            raise ValueError("observation dtype must be torch.float32 or torch.float16")
+        names = ("float32", "float16") if dtype is None else (str(dtype)[len("torch."):],)
+        return (("view", names, self.view_space[g], False), ("feature", names, self.feature_space[g], False))
+
+    def _groups(self, handle, of):                  # `of` is the group itself by default
+        g = self._hv(handle)
+        return g, g if of is None else self._hv(of)
+
+    def _outputs(self, handle, parts, slots=False, out=None, host=None):
+        """(the data of one output call's buffers for the ABI, the results, whether the call has anything to write: the
+        first buffer given holds a record).  slots: lead (num_arenas, S) and a caller's tensors of exactly that lead;
+        else lead (get_num(handle),), a caller's tensors of at least get_num_bound(handle) rows, the results trimmed to
+        the lead.  host: the name of the cached host buffers (numpy) to receive into, valid until the next call with
+        that name for the group; else CUDA tensors, new ones or the caller's `out`, checked before anything is done."""
+        lead = self._slot_shape(handle) if slots else (self.get_num(handle),)
+        if host is not None:
+            g = self._hv(handle)
+            bufs = [self._host_view((g, host, name), lead + tail, dtypes[0]) for name, dtypes, tail, _ in parts]
+            return [b.ctypes.data for b in bufs], tuple(bufs), 0 not in lead
+        import torch
+        if out is None:
+            bufs = [torch.empty(lead + tail, dtype=getattr(torch, dtypes[0]), device="cuda")
+                    for _name, dtypes, tail, _opt in parts]
+        else:
+            bufs = _out_tuple(out, parts)
+            bound = None if slots else self.get_num_bound(handle)
+            for t, (name, dtypes, tail, optional) in zip(bufs, parts):
+                _check_cuda_out(t, name if len(parts) > 1 else "out", tuple(getattr(torch, d) for d in dtypes),
+                                rows=bound, tail=tail, shape=lead + tail if slots else None, optional=optional)
+        todo = 0 not in next(t for t in bufs if t is not None).shape
+        ptrs = [None if t is None else ctypes.c_void_p(t.data_ptr()) for t in bufs]
+        return ptrs, tuple(t if slots or t is None else t[:lead[0]] for t in bufs), todo
+
     def get_action_mask(self, handle):
         """bool (n, n_action): which actions of every agent of the group would succeed if taken alone on the state as it
         is now (include/magent_b200_ext.h magent_b200_get_action_mask has the definition).  Rows are in the order of
         set_action; a dead, un-culled agent's row is all False.  The array is a cached receive buffer: valid until the
         next call."""
         g = self._hv(handle)
-        buf = self._host_view((g, "mask"), (self.get_num(handle), self.action_space[g][0]), np.uint8)
-        self._check(self._lib.magent_b200_get_action_mask(self.game, g, buf.ctypes.data), "get_action_mask")
-        return buf.view(np.bool_)
+        (ptr,), (mask,), _ = self._outputs(handle, self._mask_parts(g), host="mask")
+        self._check(self._lib.magent_b200_get_action_mask(self.game, g, ptr), "get_action_mask")
+        return mask
 
     def get_action_mask_torch(self, handle, out=None):
         """the legal-action mask (see get_action_mask) written straight into a CUDA torch.bool tensor (n, n_action):
@@ -595,15 +662,9 @@ class GridWorld(Environment):
         allocates nothing.  Returns the first get_num(handle) rows as torch.bool."""
         import torch
         g = self._hv(handle)
-        na = self.action_space[g][0]
-        n = self.get_num(handle)
-        if out is None:
-            out = torch.empty((n, na), dtype=torch.uint8, device="cuda")
-        else:
-            _check_cuda_out(out, "out", (torch.bool, torch.uint8), rows=self.get_num_bound(handle), tail=(na,))
-        self._check(self._lib.magent_b200_get_action_mask(self.game, g, ctypes.c_void_p(out.data_ptr())),
-                    "get_action_mask")
-        return out.view(torch.bool)[:n]
+        (ptr,), (mask,), _ = self._outputs(handle, self._mask_parts(g), out=out)
+        self._check(self._lib.magent_b200_get_action_mask(self.game, g, ptr), "get_action_mask")
+        return mask.view(torch.bool)
 
     def set_random_legal_actions(self, handle, seed):
         """set_action with an action drawn uniformly from every agent's legal actions (get_action_mask), on the device:
@@ -617,15 +678,10 @@ class GridWorld(Environment):
         Q-learning's neighbour action (include/magent_b200_ext.h magent_b200_get_mean_action has the definition).  Called
         after step and before the next set_action it gives the previous step's actions.  Rows are in the order of
         set_action.  Both arrays are cached receive buffers: valid until the next call."""
-        g = self._hv(handle)
-        o = g if of is None else self._hv(of)
-        n = self.get_num(handle)
-        na = self.action_space[o][0]
-        raw = self._host_view((g, "mean"), (n * (na + 1),), np.float32)
-        mean, count = raw[:n * na].reshape(n, na), raw[n * na:].view(np.int32)
-        self._check(self._lib.magent_b200_get_mean_action(self.game, g, o, mean.ctypes.data, count.ctypes.data),
-                    "get_mean_action")
-        return mean, count
+        g, o = self._groups(handle, of)
+        ptrs, res, _ = self._outputs(handle, self._mean_parts(o), host="mean")
+        self._check(self._lib.magent_b200_get_mean_action(self.game, g, o, *ptrs), "get_mean_action")
+        return res
 
     def get_mean_action_torch(self, handle, of=None, out=None):
         """the mean neighbour action (see get_mean_action) written straight into CUDA tensors: returns (mean float32
@@ -634,24 +690,10 @@ class GridWorld(Environment):
         out: a caller-owned pair (mean, count) of contiguous CUDA tensors, float32 (rows, n_action(of)) and int32
         (rows,), with at least get_num_bound(handle) rows each; needed to record the call into a CUDA graph
         (capture_graph), since the call then allocates nothing.  Returns the first get_num(handle) rows of each."""
-        import torch
-        g = self._hv(handle)
-        o = g if of is None else self._hv(of)
-        na = self.action_space[o][0]
-        n = self.get_num(handle)
-        if out is None:
-            mean = torch.empty((n, na), dtype=torch.float32, device="cuda")
-            count = torch.empty((n,), dtype=torch.int32, device="cuda")
-        else:
-            if not isinstance(out, (tuple, list)) or len(out) != 2:
-                raise ValueError("out must be a (mean, count) pair of CUDA tensors")
-            mean, count = out
-            bound = self.get_num_bound(handle)
-            _check_cuda_out(mean, "mean", (torch.float32,), rows=bound, tail=(na,))
-            _check_cuda_out(count, "count", (torch.int32,), rows=bound)
-        self._check(self._lib.magent_b200_get_mean_action(self.game, g, o, ctypes.c_void_p(mean.data_ptr()),
-                                                          ctypes.c_void_p(count.data_ptr())), "get_mean_action")
-        return mean[:n], count[:n]
+        g, o = self._groups(handle, of)
+        ptrs, res, _ = self._outputs(handle, self._mean_parts(o), out=out)
+        self._check(self._lib.magent_b200_get_mean_action(self.game, g, o, *ptrs), "get_mean_action")
+        return res
 
     def get_neighbours(self, handle, k, of=None):
         """(idx int32 (n, k), rel int32 (n, k, 2), count int32 (n,)): for every agent of the group, the first k of the
@@ -660,17 +702,11 @@ class GridWorld(Environment):
         definition).  idx: their rows in group `of`'s order (get_pos(of), get_observation(of)), rel: the (vy, vx) view
         cell where the observer's own observation shows them, count: how many neighbours it has in all.  Unused slots
         are -1.  Rows are in the order of set_action.  The arrays are cached receive buffers: valid until the next call."""
-        g = self._hv(handle)
-        o = g if of is None else self._hv(of)
-        k = int(k)
-        if not 1 <= k <= 32:
-            raise ValueError("k must be in [1, 32], got %d" % k)
-        n = self.get_num(handle)
-        raw = self._host_view((g, "nbr"), (n * (3 * k + 1),), np.int32)
-        idx, rel, count = raw[:n * k].reshape(n, k), raw[n * k:3 * n * k].reshape(n, k, 2), raw[3 * n * k:]
-        self._check(self._lib.magent_b200_get_neighbours(self.game, g, o, k, idx.ctypes.data, rel.ctypes.data,
-                                                         count.ctypes.data), "get_neighbours")
-        return idx, rel, count
+        g, o = self._groups(handle, of)
+        k, parts = self._nbr_parts(k)
+        ptrs, res, _ = self._outputs(handle, parts, host="nbr")
+        self._check(self._lib.magent_b200_get_neighbours(self.game, g, o, k, *ptrs), "get_neighbours")
+        return res
 
     def get_neighbours_torch(self, handle, k, of=None, out=None):
         """the nearest visible neighbours (see get_neighbours) written straight into CUDA tensors: returns (idx int32
@@ -681,30 +717,12 @@ class GridWorld(Environment):
         (capture_graph), since the call then allocates nothing.  rel and count may be None: they are then neither
         computed nor written (without count the kernel stops at the k-th neighbour), and None comes back in their place.
         Returns the first get_num(handle) rows of each."""
-        import torch
-        g = self._hv(handle)
-        o = g if of is None else self._hv(of)
-        k = int(k)
-        if not 1 <= k <= 32:
-            raise ValueError("k must be in [1, 32], got %d" % k)
-        n = self.get_num(handle)
-        if out is None:
-            idx = torch.empty((n, k), dtype=torch.int32, device="cuda")
-            rel = torch.empty((n, k, 2), dtype=torch.int32, device="cuda")
-            count = torch.empty((n,), dtype=torch.int32, device="cuda")
-        else:
-            if not isinstance(out, (tuple, list)) or len(out) != 3:
-                raise ValueError("out must be an (idx, rel, count) triple of CUDA tensors")
-            idx, rel, count = out
-            bound = self.get_num_bound(handle)
-            _check_cuda_out(idx, "idx", (torch.int32,), rows=bound, tail=(k,))
-            _check_cuda_out(rel, "rel", (torch.int32,), rows=bound, tail=(k, 2), optional=True)
-            _check_cuda_out(count, "count", (torch.int32,), rows=bound, optional=True)
-        if idx.shape[0] == 0:            # no row can be written (num_bound is 0), and an empty tensor's pointer is NULL
-            return idx, rel, count
-        self._check(self._lib.magent_b200_get_neighbours(self.game, g, o, k, _dptr(idx), _dptr(rel), _dptr(count)),
-                    "get_neighbours")
-        return idx[:n], None if rel is None else rel[:n], None if count is None else count[:n]
+        g, o = self._groups(handle, of)
+        k, parts = self._nbr_parts(k)
+        ptrs, res, todo = self._outputs(handle, parts, out=out)
+        if todo:            # no row can be written, and the engine refuses the NULL data of an empty idx
+            self._check(self._lib.magent_b200_get_neighbours(self.game, g, o, k, *ptrs), "get_neighbours")
+        return res
 
     def get_slot_space(self, handle):
         """S, the slot space of the group: slots run over [0, S) in every arena (include/magent_b200_ext.h
@@ -765,13 +783,11 @@ class GridWorld(Environment):
         the record get_observation gives the row slot_row[a, s]; a vacant slot is all zeros.  The arrays are cached
         receive buffers: valid until the next call."""
         g = self._hv(handle)
-        lead = (self.num_arenas, self.get_slot_space(handle))
-        view = self._host_view((g, "view_slots"), lead + self.view_space[g], np.float32)
-        feat = self._host_view((g, "feature_slots"), lead + self.feature_space[g], np.float32)
-        if view.size:
-            bufs = (ctypes.c_void_p * 2)(view.ctypes.data, feat.ctypes.data)
-            self._check(self._lib.magent_b200_get_observation_slots(self.game, g, bufs, 0), "get_observation_slots")
-        return view, feat
+        ptrs, res, todo = self._outputs(handle, self._obs_parts(g), slots=True, host="obs_slots")
+        if todo:
+            self._check(self._lib.magent_b200_get_observation_slots(self.game, g, (ctypes.c_void_p * 2)(*ptrs), 0),
+                        "get_observation_slots")
+        return res
 
     def get_observation_slots_torch(self, handle, out=None, dtype=None):
         """the slot-ordered observation (see get_observation_slots) rendered straight into CUDA tensors, without waiting
@@ -783,23 +799,11 @@ class GridWorld(Environment):
         run."""
         import torch
         g = self._hv(handle)
-        lead = (self.num_arenas, self.get_slot_space(handle))
-        shapes = (lead + self.view_space[g], lead + self.feature_space[g])
-        if out is None:
-            dtype = torch.float32 if dtype is None else dtype
-            if dtype not in (torch.float32, torch.float16):
-                raise ValueError("observation dtype must be torch.float32 or torch.float16")
-            view, feat = (torch.empty(s, dtype=dtype, device="cuda") for s in shapes)
-        else:
-            if not isinstance(out, (tuple, list)) or len(out) != 2:
-                raise ValueError("out must be a (view, feature) pair of CUDA tensors")
-            view, feat = out
-            dtypes = (torch.float32, torch.float16) if dtype is None else (dtype,)
-            _check_cuda_out(view, "view", dtypes, shape=shapes[0])
-            _check_cuda_out(feat, "feature", (view.dtype,), shape=shapes[1])
-        if view.numel():
-            bufs = (ctypes.c_void_p * 2)(view.data_ptr(), feat.data_ptr())
-            self._check(self._lib.magent_b200_get_observation_slots(self.game, g, bufs,
+        ptrs, (view, feat), todo = self._outputs(handle, self._obs_parts(g, dtype), slots=True, out=out)
+        if feat.dtype != view.dtype:
+            raise ValueError("view and feature must be of one dtype, not %s and %s" % (view.dtype, feat.dtype))
+        if todo:
+            self._check(self._lib.magent_b200_get_observation_slots(self.game, g, (ctypes.c_void_p * 2)(*ptrs),
                                                                     1 if view.dtype == torch.float16 else 0),
                         "get_observation_slots")
         return view, feat
@@ -831,13 +835,10 @@ class GridWorld(Environment):
         is the per-agent terminal signal); +0.0 and 0 in vacant slots.  Both arrays are cached receive buffers: valid
         until the next call."""
         g = self._hv(handle)
-        shape = self._slot_shape(handle)
-        reward = self._host_view((g, "reward_slots"), shape, np.float32)
-        status = self._host_view((g, "status_slots"), shape, np.uint8)
-        if reward.size:
-            self._check(self._lib.magent_b200_get_reward_slots(self.game, g, reward.ctypes.data, status.ctypes.data),
-                        "get_reward_slots")
-        return reward, status
+        ptrs, res, todo = self._outputs(handle, self._REWARD_PARTS, slots=True, host="reward_slots")
+        if todo:
+            self._check(self._lib.magent_b200_get_reward_slots(self.game, g, *ptrs), "get_reward_slots")
+        return res
 
     def get_reward_slots_torch(self, handle, out=None):
         """the slot-ordered reward and status (see get_reward_slots) written straight into CUDA tensors, without waiting
@@ -846,33 +847,21 @@ class GridWorld(Environment):
         out: a caller-owned pair (reward, status) of contiguous CUDA tensors of those shapes and dtypes; needed to record
         the call into a CUDA graph (capture_graph), since the call then allocates nothing.  Either may be None: it is
         then not written, and None comes back in its place."""
-        import torch
         g = self._hv(handle)
-        shape = self._slot_shape(handle)
-        if out is None:
-            reward = torch.empty(shape, dtype=torch.float32, device="cuda")
-            status = torch.empty(shape, dtype=torch.uint8, device="cuda")
-        else:
-            if not isinstance(out, (tuple, list)) or len(out) != 2 or (out[0] is None and out[1] is None):
-                raise ValueError("out must be a (reward, status) pair of CUDA tensors, at most one of them None")
-            reward, status = out
-            _check_cuda_out(reward, "reward", (torch.float32,), shape=shape, optional=True)
-            _check_cuda_out(status, "status", (torch.uint8,), shape=shape, optional=True)
-        if shape[1]:
-            self._check(self._lib.magent_b200_get_reward_slots(self.game, g, _dptr(reward), _dptr(status)),
-                        "get_reward_slots")
-        return reward, status
+        ptrs, res, todo = self._outputs(handle, self._REWARD_PARTS, slots=True, out=out)
+        if todo:
+            self._check(self._lib.magent_b200_get_reward_slots(self.game, g, *ptrs), "get_reward_slots")
+        return res
 
     def get_action_mask_slots(self, handle):
         """bool (num_arenas, S, n_action): the legal-action mask (see get_action_mask) in the stable slot layout; all
         False in vacant slots and for dead, un-culled agents.  The array is a cached receive buffer: valid until the next
         call."""
         g = self._hv(handle)
-        buf = self._host_view((g, "mask_slots"), self._slot_shape(handle) + (self.action_space[g][0],), np.uint8)
-        if buf.size:
-            self._check(self._lib.magent_b200_get_action_mask_slots(self.game, g, buf.ctypes.data),
-                        "get_action_mask_slots")
-        return buf.view(np.bool_)
+        (ptr,), (mask,), todo = self._outputs(handle, self._mask_parts(g), slots=True, host="mask_slots")
+        if todo:
+            self._check(self._lib.magent_b200_get_action_mask_slots(self.game, g, ptr), "get_action_mask_slots")
+        return mask
 
     def get_action_mask_slots_torch(self, handle, out=None):
         """the slot-ordered legal-action mask (see get_action_mask_slots) written straight into a CUDA torch.bool tensor
@@ -882,29 +871,20 @@ class GridWorld(Environment):
         into a CUDA graph (capture_graph), since the call then allocates nothing once a first call has run."""
         import torch
         g = self._hv(handle)
-        shape = self._slot_shape(handle) + (self.action_space[g][0],)
-        if out is None:
-            out = torch.empty(shape, dtype=torch.uint8, device="cuda")
-        else:
-            _check_cuda_out(out, "out", (torch.bool, torch.uint8), shape=shape)
-        if out.numel():
-            self._check(self._lib.magent_b200_get_action_mask_slots(self.game, g, ctypes.c_void_p(out.data_ptr())),
-                        "get_action_mask_slots")
-        return out.view(torch.bool)
+        (ptr,), (mask,), todo = self._outputs(handle, self._mask_parts(g), slots=True, out=out)
+        if todo:
+            self._check(self._lib.magent_b200_get_action_mask_slots(self.game, g, ptr), "get_action_mask_slots")
+        return mask.view(torch.bool)
 
     def get_mean_action_slots(self, handle, of=None):
         """(mean float32 (num_arenas, S, n_action(of)), count int32 (num_arenas, S)): the mean neighbour action (see
         get_mean_action) in the stable slot layout (see get_slots); a +0.0 row and count 0 in vacant slots.  Both arrays
         are cached receive buffers: valid until the next call."""
-        g = self._hv(handle)
-        o = g if of is None else self._hv(of)
-        shape = self._slot_shape(handle)
-        mean = self._host_view((g, "mean_slots"), shape + (self.action_space[o][0],), np.float32)
-        count = self._host_view((g, "mean_count_slots"), shape, np.int32)
-        if count.size:
-            self._check(self._lib.magent_b200_get_mean_action_slots(self.game, g, o, mean.ctypes.data,
-                                                                    count.ctypes.data), "get_mean_action_slots")
-        return mean, count
+        g, o = self._groups(handle, of)
+        ptrs, res, todo = self._outputs(handle, self._mean_parts(o, slots=True), slots=True, host="mean_slots")
+        if todo:
+            self._check(self._lib.magent_b200_get_mean_action_slots(self.game, g, o, *ptrs), "get_mean_action_slots")
+        return res
 
     def get_mean_action_slots_torch(self, handle, of=None, out=None):
         """the slot-ordered mean neighbour action (see get_mean_action_slots) written straight into CUDA tensors, without
@@ -913,24 +893,11 @@ class GridWorld(Environment):
         out: a caller-owned pair (mean, count) of contiguous CUDA tensors of those shapes and dtypes; needed to record
         the call into a CUDA graph (capture_graph), since the call then allocates nothing once a first call has run.
         count may be None: it is then not written, and None comes back in its place."""
-        import torch
-        g = self._hv(handle)
-        o = g if of is None else self._hv(of)
-        shape = self._slot_shape(handle)
-        mshape = shape + (self.action_space[o][0],)
-        if out is None:
-            mean = torch.empty(mshape, dtype=torch.float32, device="cuda")
-            count = torch.empty(shape, dtype=torch.int32, device="cuda")
-        else:
-            if not isinstance(out, (tuple, list)) or len(out) != 2:
-                raise ValueError("out must be a (mean, count) pair of CUDA tensors, count possibly None")
-            mean, count = out
-            _check_cuda_out(mean, "mean", (torch.float32,), shape=mshape)
-            _check_cuda_out(count, "count", (torch.int32,), shape=shape, optional=True)
-        if shape[1]:
-            self._check(self._lib.magent_b200_get_mean_action_slots(self.game, g, o, _dptr(mean), _dptr(count)),
-                        "get_mean_action_slots")
-        return mean, count
+        g, o = self._groups(handle, of)
+        ptrs, res, todo = self._outputs(handle, self._mean_parts(o, slots=True), slots=True, out=out)
+        if todo:
+            self._check(self._lib.magent_b200_get_mean_action_slots(self.game, g, o, *ptrs), "get_mean_action_slots")
+        return res
 
     def get_neighbours_slots(self, handle, k, of=None):
         """(idx int32 (num_arenas, S, k), rel int32 (num_arenas, S, k, 2), count int32 (num_arenas, S)): the nearest
@@ -938,19 +905,12 @@ class GridWorld(Environment):
         flat slot a * S_of + slot in group `of` (S_of = get_slot_space(of)) instead of its row, so it stays valid for the
         episode: after clear_dead it may name a vacant slot, never another agent.  Unused entries and vacant slots are
         -1, with count 0.  The arrays are cached receive buffers: valid until the next call."""
-        g = self._hv(handle)
-        o = g if of is None else self._hv(of)
-        k = int(k)
-        if not 1 <= k <= 32:
-            raise ValueError("k must be in [1, 32], got %d" % k)
-        shape = self._slot_shape(handle)
-        idx = self._host_view((g, "nbr_idx_slots"), shape + (k,), np.int32)
-        rel = self._host_view((g, "nbr_rel_slots"), shape + (k, 2), np.int32)
-        count = self._host_view((g, "nbr_count_slots"), shape, np.int32)
-        if count.size:
-            self._check(self._lib.magent_b200_get_neighbours_slots(self.game, g, o, k, idx.ctypes.data, rel.ctypes.data,
-                                                                   count.ctypes.data), "get_neighbours_slots")
-        return idx, rel, count
+        g, o = self._groups(handle, of)
+        k, parts = self._nbr_parts(k)
+        ptrs, res, todo = self._outputs(handle, parts, slots=True, host="nbr_slots")
+        if todo:
+            self._check(self._lib.magent_b200_get_neighbours_slots(self.game, g, o, k, *ptrs), "get_neighbours_slots")
+        return res
 
     def get_neighbours_slots_torch(self, handle, k, of=None, out=None):
         """the slot-ordered nearest visible neighbours (see get_neighbours_slots) written straight into CUDA tensors,
@@ -961,28 +921,12 @@ class GridWorld(Environment):
         the call into a CUDA graph (capture_graph), since the call then allocates nothing once a first call has run.  rel
         and count may be None: they are then neither computed nor written (without count the kernel stops at the k-th
         neighbour), and None comes back in their place."""
-        import torch
-        g = self._hv(handle)
-        o = g if of is None else self._hv(of)
-        k = int(k)
-        if not 1 <= k <= 32:
-            raise ValueError("k must be in [1, 32], got %d" % k)
-        shape = self._slot_shape(handle)
-        if out is None:
-            idx = torch.empty(shape + (k,), dtype=torch.int32, device="cuda")
-            rel = torch.empty(shape + (k, 2), dtype=torch.int32, device="cuda")
-            count = torch.empty(shape, dtype=torch.int32, device="cuda")
-        else:
-            if not isinstance(out, (tuple, list)) or len(out) != 3:
-                raise ValueError("out must be an (idx, rel, count) triple of CUDA tensors")
-            idx, rel, count = out
-            _check_cuda_out(idx, "idx", (torch.int32,), shape=shape + (k,))
-            _check_cuda_out(rel, "rel", (torch.int32,), shape=shape + (k, 2), optional=True)
-            _check_cuda_out(count, "count", (torch.int32,), shape=shape, optional=True)
-        if shape[1]:
-            self._check(self._lib.magent_b200_get_neighbours_slots(self.game, g, o, k, _dptr(idx), _dptr(rel),
-                                                                   _dptr(count)), "get_neighbours_slots")
-        return idx, rel, count
+        g, o = self._groups(handle, of)
+        k, parts = self._nbr_parts(k)
+        ptrs, res, todo = self._outputs(handle, parts, slots=True, out=out)
+        if todo:
+            self._check(self._lib.magent_b200_get_neighbours_slots(self.game, g, o, k, *ptrs), "get_neighbours_slots")
+        return res
 
     # ---- built-in scripted opponents (include/magent_b200_ext.h magent_b200_rule_actions has the definition)
     RULE_POLICIES = {"rush": 0, "flee": 1}
@@ -1005,11 +949,10 @@ class GridWorld(Environment):
     def get_rule_actions(self, handle, target, policy="rush", seed=0):
         """int32 (n,): the actions set_rule_actions would set, in the order of set_action.  The array is a cached
         receive buffer: valid until the next call."""
-        g = self._hv(handle)
-        buf = self._host_view((g, "rule"), (self.get_num(handle),), np.int32)
+        (ptr,), (act,), todo = self._outputs(handle, self._RULE_PARTS, host="rule")
         self._check(self._lib.magent_b200_get_rule_actions(*self._rule_args(handle, target, policy, seed),
-                                                           buf.ctypes.data if buf.size else None), "get_rule_actions")
-        return buf
+                                                           ptr if todo else None), "get_rule_actions")
+        return act
 
     def get_rule_actions_torch(self, handle, target, policy="rush", seed=0, out=None):
         """the scripted actions (see get_rule_actions) written straight into a CUDA int32 tensor (n,).
@@ -1017,26 +960,19 @@ class GridWorld(Environment):
         out: a caller-owned contiguous CUDA int32 tensor (rows,) with at least get_num_bound(handle) rows; needed to
         record the call into a CUDA graph (capture_graph), since the call then allocates nothing.  Returns its first
         get_num(handle) entries."""
-        import torch
-        n = self.get_num(handle)
-        if out is None:
-            out = torch.empty((n,), dtype=torch.int32, device="cuda")
-        else:
-            _check_cuda_out(out, "out", (torch.int32,), rows=self.get_num_bound(handle))
-        if out.numel():
-            self._check(self._lib.magent_b200_get_rule_actions(*self._rule_args(handle, target, policy, seed),
-                                                               _dptr(out)), "get_rule_actions")
-        return out[:n]
+        (ptr,), (act,), todo = self._outputs(handle, self._RULE_PARTS, out=out)
+        if todo:
+            self._check(self._lib.magent_b200_get_rule_actions(*self._rule_args(handle, target, policy, seed), ptr),
+                        "get_rule_actions")
+        return act
 
     def get_rule_actions_slots(self, handle, target, policy="rush", seed=0):
         """int32 (num_arenas, S): the scripted actions (see get_rule_actions) in the stable slot layout (see get_slots);
         -1 in vacant slots.  The array is a cached receive buffer: valid until the next call."""
-        g = self._hv(handle)
-        buf = self._host_view((g, "rule_slots"), self._slot_shape(handle), np.int32)
+        (ptr,), (act,), todo = self._outputs(handle, self._RULE_PARTS, slots=True, host="rule_slots")
         self._check(self._lib.magent_b200_get_rule_actions_slots(*self._rule_args(handle, target, policy, seed),
-                                                                 buf.ctypes.data if buf.size else None),
-                    "get_rule_actions_slots")
-        return buf
+                                                                 ptr if todo else None), "get_rule_actions_slots")
+        return act
 
     def get_rule_actions_slots_torch(self, handle, target, policy="rush", seed=0, out=None):
         """the slot-ordered scripted actions (see get_rule_actions_slots) written straight into a CUDA int32 tensor
@@ -1044,15 +980,10 @@ class GridWorld(Environment):
 
         out: a caller-owned contiguous CUDA int32 tensor of that shape; needed to record the call into a CUDA graph
         (capture_graph), since the call then allocates nothing once a first call has run."""
-        import torch
-        shape = self._slot_shape(handle)
-        if out is None:
-            out = torch.empty(shape, dtype=torch.int32, device="cuda")
-        else:
-            _check_cuda_out(out, "out", (torch.int32,), shape=shape)
+        (ptr,), (act,), todo = self._outputs(handle, self._RULE_PARTS, slots=True, out=out)
         self._check(self._lib.magent_b200_get_rule_actions_slots(*self._rule_args(handle, target, policy, seed),
-                                                                 _dptr(out)), "get_rule_actions_slots")
-        return out
+                                                                 ptr if todo else None), "get_rule_actions_slots")
+        return act
 
     def get_counters(self):
         """int64 event counters accumulated on the device since construction"""
