@@ -273,6 +273,30 @@ int magent_b200_free_snapshot(EnvHandle game, int snapshot);
  * "num_bound".  env_get_info(game, -1, "arena_rng", uint32[num_arenas]) gives each arena's minstd state (a value for
  * the "seed" key would have to be this to continue the stream). */
 int magent_b200_restore_arenas(EnvHandle game, int snapshot, const int *src, int keep_rng);
+/* replay recorder: watch chosen arenas of a device-resident loop in the reference viewer's replay format.  The calls
+ * below return -1 and set magent_b200_last_error when they refuse; the state is then unchanged.
+ *
+ * replay_new makes a recorder of arenas[0, n_arenas) (distinct, in [0, num_arenas)) with room for max_frames (>= 1)
+ * frames on the device and returns its id (>= 0).  Refused during a CUDA graph capture and after the game has captured
+ * any graph: steps captured without a live recorder do not record attack events, so make recorders before capturing.
+ * replay_record appends one frame per arena of the recorder: what env_render would write at that point with
+ * magent_b200_select_arena(a) in force ("F num_agents n_attack 0", the agent lines "id hp angle x y group" in group and
+ * row order with un-culled dead agents listed and un-absorbed absorbers skipped, then the attack events of the arena's
+ * last env_step in execution order as "0 id x y"; a restored arena has none until its next step).  It neither
+ * synchronises nor allocates, so it can be recorded into a CUDA graph.  With max_frames frames buffered the frame is
+ * dropped and counted.  Refused when the per-arena agent bound has grown past what the frames were sized for.
+ * replay_write synchronises, writes dir/arena_<a>/config.json (the bytes env_render writes) and appends the buffered
+ * frames to dir/arena_<a>/video_<k>.txt, then empties the buffer: it returns the number of frames per arena written and
+ * the frames dropped since the last write into *dropped (may be NULL).  A file starts with the "W" wall block; a new one
+ * opens at the first frame of each episode of the arena (env_reset, or a restore_arenas that replaces it, also from
+ * itself; src[a] = -1 does not) starting with video_1.txt, and after 10 000 frames as env_render splits them.  Two
+ * writes give the bytes of one.  replay_free releases a recorder; one recorded into a captured graph lives as long as
+ * the game.  While a recorder is live every step also collects the attack events of the recorded arenas; all other
+ * outputs stay bit-identical, and restore_arenas and graph capture are not refused (env_render still refuses them). */
+int magent_b200_replay_new(EnvHandle game, const int *arenas, int n_arenas, int max_frames);
+int magent_b200_replay_record(EnvHandle game, int replay);
+int magent_b200_replay_write(EnvHandle game, int replay, const char *dir, long long *dropped);
+int magent_b200_replay_free(EnvHandle game, int replay);
 /* per-arena done flags of the last env_step into int32[num_arenas], host or CUDA device pointer; with a device pointer
  * nothing is waited for */
 int magent_b200_get_arena_done(EnvHandle game, int *out);

@@ -83,6 +83,10 @@ EXT_SIGNATURES = {
     "magent_b200_snapshot_arenas": ([_vp], ctypes.c_int),
     "magent_b200_free_snapshot": ([_vp, ctypes.c_int], ctypes.c_int),
     "magent_b200_restore_arenas": ([_vp, ctypes.c_int, _vp, ctypes.c_int], ctypes.c_int),
+    "magent_b200_replay_new": ([_vp, _vp, ctypes.c_int, ctypes.c_int], ctypes.c_int),
+    "magent_b200_replay_record": ([_vp, ctypes.c_int], ctypes.c_int),
+    "magent_b200_replay_write": ([_vp, ctypes.c_int, ctypes.c_char_p, _vp], ctypes.c_int),
+    "magent_b200_replay_free": ([_vp, ctypes.c_int], ctypes.c_int),
     "magent_b200_get_arena_done": ([_vp, _vp], ctypes.c_int),
     "magent_b200_get_counters": ([_vp, ctypes.POINTER(ctypes.c_longlong), ctypes.c_int], ctypes.c_int),
     "magent_b200_last_error": ([], ctypes.c_char_p),

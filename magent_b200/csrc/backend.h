@@ -152,6 +152,30 @@ __attribute__((weak)) void launch_rule_actions(Ctx *, const EngineDev *dE, const
 __attribute__((weak)) void launch_rule_actions_slots(Ctx *, const EngineDev *dE, const EngineDev &hE, const SlotDev *T,
                                                      const NbrCell *lut, unsigned curmask, int group, int target,
                                                      int policy, unsigned long long seed, int S, int *out);
+// The replay recorder (replay_phases.h; Engine::replay_new).  None of these synchronises or allocates.
+// launch_replay_events: right after a launch_step with StepArgs::record_events, for each arena a of arenas[0, n_arenas)
+// (a device buffer; entries < 0 are skipped): rep[a].ev_n[g] = the device-side count of group g, and for every row i
+// below it ev[a * hE.cap_total + foff(g) + i] = replay_event of the row (rank: its GroupDev::ev_rank).
+// launch_replay_restore: for every arena launch_restore (same src and done rules) is about to replace, rep[a].episode
+// += 1 and every rep[a].ev_n = 0; it runs before launch_restore, which changes the done words.
+// launch_replay_record: one frame (RepLayout R.L) of each arena R.arenas[k] into frame R.ctl->n_frames, slot k: header
+// {episode, walls present, device-side counts, rep ev_n}, the RepAgent of every row, the event rows below ev_n, and the
+// wall bitmap of occ when the episode differs from R.last_ep[k]; then n_frames += 1 and last_ep[k] = episode.  With
+// R.max_frames frames buffered nothing is written and R.ctl->dropped += 1.  Weak like launch_slots: the engine refuses
+// the recorder without them.
+struct RepRecord {
+    const int *arenas;                       // [n_arenas], device
+    int n_arenas, max_frames;
+    RepLayout L;
+    int *frames;                             // [max_frames][n_arenas][L.frame_ints()]
+    int *last_ep;                            // [n_arenas]
+    RepCtl *ctl;
+};
+__attribute__((weak)) void launch_replay_events(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask,
+                                                RepArena *rep, RepEvent *ev, const int *arenas, int n_arenas);
+__attribute__((weak)) void launch_replay_restore(Ctx *, const EngineDev &hE, RepArena *rep, const int *src);
+__attribute__((weak)) void launch_replay_record(Ctx *, const EngineDev *dE, const EngineDev &hE, unsigned curmask,
+                                                const RepArena *rep, const RepEvent *ev, const RepRecord &R);
 // Whether kernel `which` fits the device's shared memory for `group` (and, for the mean action, the histograms of group
 // `of`'s actions): its static shared memory plus what the view or the action space asks for, against the device's
 // opt-in limit per block (the default limit for the wire kernel, which does not opt in).  When it does not, *why (unless

@@ -31,6 +31,7 @@ namespace mg { __device__ long long mg_phase_clock[8 * 32]; }
 #include "nbr_phases.h"
 #include "rule_phases.h"
 #include "slot_phases.h"
+#include "replay_phases.h"
 
 namespace cg = cooperative_groups;
 
@@ -3004,6 +3005,130 @@ void launch_rule_actions_slots(Ctx *c, const EngineDev *dE, const EngineDev &hE,
     rule_actions_slots_kernel<<<(unsigned)((size_t)hE.A * cps), RULE_THREADS, 0, c->stream>>>(
         dE, lut, curmask, group, target, policy, seed, c->obs_slot_row, S, out, cps);
     post_launch("rule_actions_slots_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
+// replay recorder (replay_phases.h).  Every kernel covers agents, not arenas: a thread per flat row (GroupDev::foff + i)
+// of a recorded arena, blockIdx.y the arena, so one arena of 800k agents spreads over the whole GPU like 64 small ones.
+constexpr int REP_THREADS = 256;
+constexpr unsigned REP_MAX_Y = 65535;
+
+__global__ void __launch_bounds__(REP_THREADS) replay_events_kernel(const EngineDev *gE, unsigned curmask, RepArena *rep,
+                                                                    RepEvent *ev, const int *arenas, int n_arenas) {
+    const EngineDev &E = *gE;
+    const int f = blockIdx.x * REP_THREADS + threadIdx.x;
+    if (f >= E.cap_total) return;
+    const int g = replay_group_of(E, f);
+    if (g < 0) return;
+    const GroupDev &G = E.grp[g];
+    const int i = f - G.foff;
+    const AgentSoA &s = G.soa[(curmask >> g) & 1u];
+    for (int k = blockIdx.y; k < n_arenas; k += gridDim.y) {
+        const int a = __ldg(arenas + k);
+        if (a < 0) continue;
+        const int n = E.n[(long)g * E.A + a];
+        if (i == 0) rep[a].ev_n[g] = n;
+        if (i >= n) continue;
+        const long gi = (long)a * G.cap + i;
+        ev[(long)a * E.cap_total + f] = replay_event(G, s, E.turn_mode, gi, G.ev_rank[gi]);
+    }
+}
+
+void launch_replay_events(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curmask, RepArena *rep,
+                          RepEvent *ev, const int *arenas, int n_arenas) {
+    if (n_arenas <= 0 || hE.cap_total <= 0) return;
+    DeviceGuard guard(c);
+    const dim3 grid((unsigned)((hE.cap_total + REP_THREADS - 1) / REP_THREADS), std::min((unsigned)n_arenas, REP_MAX_Y));
+    replay_events_kernel<<<grid, REP_THREADS, 0, c->stream>>>(dE, curmask, rep, ev, arenas, n_arenas);
+    post_launch("replay_events_kernel");
+}
+
+__global__ void __launch_bounds__(REP_THREADS) replay_restore_kernel(RepArena *rep, const int *src, const int *done, int A) {
+    const int a = blockIdx.x * REP_THREADS + threadIdx.x;
+    if (a >= A || restore_source(src, done, A, a) < 0) return;
+    rep[a].episode += 1;
+    for (int g = 0; g < MG_MAX_GROUPS; ++g) rep[a].ev_n[g] = 0;
+}
+
+void launch_replay_restore(Ctx *c, const EngineDev &hE, RepArena *rep, const int *src) {
+    DeviceGuard guard(c);
+    replay_restore_kernel<<<(unsigned)((hE.A + REP_THREADS - 1) / REP_THREADS), REP_THREADS, 0, c->stream>>>(rep, src, hE.done, hE.A);
+    post_launch("replay_restore_kernel");
+}
+
+// items of a recorded arena: cap_total agent rows, cap_total event rows, wall_words bitmap words.  Every CTA reads the
+// frame counter and the last episodes first; the last CTA to finish (ticket) advances them, so no CTA of this launch
+// sees them change.
+__global__ void __launch_bounds__(REP_THREADS) replay_record_kernel(const EngineDev *gE, unsigned curmask,
+                                                                    const RepArena *rep, const RepEvent *ev,
+                                                                    const RepRecord R) {
+    const EngineDev &E = *gE;
+    const int frame = *(volatile const int *)&R.ctl->n_frames;
+    if (frame < R.max_frames) {
+        const int item = blockIdx.x * REP_THREADS + threadIdx.x;
+        const int ct = R.L.cap_total;
+        const long cells = (long)E.W * E.H;
+        const long agent_base = R.L.agent_base(), event_base = R.L.event_base(), wall_base = R.L.wall_base();
+        const long frame_ints = R.L.frame_ints();
+        for (int k = blockIdx.y; k < R.n_arenas; k += gridDim.y) {
+            const int a = __ldg(R.arenas + k);
+            const int episode = rep[a].episode;
+            const bool walls = episode != R.last_ep[k];
+            int *F = R.frames + ((long)frame * R.n_arenas + k) * frame_ints;
+            if (item == 0) {
+                F[REP_H_EPISODE] = episode;
+                F[REP_H_WALLS] = walls ? 1 : 0;
+                for (int g = 0; g < MG_MAX_GROUPS; ++g) {
+                    F[REP_H_N + g] = g < E.G ? E.n[(long)g * E.A + a] : 0;
+                    F[REP_H_EV_N + g] = g < E.G ? rep[a].ev_n[g] : 0;
+                }
+            }
+            if (item < 2 * ct) {
+                const int f = item < ct ? item : item - ct;
+                const int g = replay_group_of(E, f);
+                if (g < 0) continue;
+                const GroupDev &G = E.grp[g];
+                const int i = f - G.foff;
+                if (item < ct) {
+                    if (i >= E.n[(long)g * E.A + a]) continue;
+                    const RepAgent r = replay_agent(G.soa[(curmask >> g) & 1u], E.turn_mode, (long)a * G.cap + i);
+                    int *o = F + agent_base + (long)f * (sizeof(RepAgent) / 4);
+                    o[0] = r.id; o[1] = r.x; o[2] = r.y; o[3] = __float_as_int(r.hp); o[4] = r.dir_flags;
+                } else {
+                    if (i >= rep[a].ev_n[g]) continue;
+                    const int4 e = *reinterpret_cast<const int4 *>(ev + (long)a * ct + f);
+                    reinterpret_cast<int4 *>(F + event_base)[f] = e;
+                }
+            } else if (walls && item - 2 * ct < R.L.wall_words) {
+                const int w = item - 2 * ct;
+                F[wall_base + w] = (int)replay_wall_word(E.occ + (long)a * cells, cells, w);
+            }
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        const unsigned last = gridDim.x * gridDim.y - 1;
+        if (atomicAdd(&R.ctl->ticket, 1u) == last) {
+            if (frame < R.max_frames) {
+                for (int k = 0; k < R.n_arenas; ++k) R.last_ep[k] = rep[__ldg(R.arenas + k)].episode;
+                R.ctl->n_frames = frame + 1;
+            } else {
+                R.ctl->dropped += 1;
+            }
+            R.ctl->ticket = 0;
+            __threadfence();
+        }
+    }
+}
+
+void launch_replay_record(Ctx *c, const EngineDev *dE, const EngineDev &hE, unsigned curmask, const RepArena *rep,
+                          const RepEvent *ev, const RepRecord &R) {
+    DeviceGuard guard(c);
+    const long items = 2L * R.L.cap_total + R.L.wall_words;
+    const dim3 grid((unsigned)std::max(1L, (items + REP_THREADS - 1) / REP_THREADS), std::min((unsigned)R.n_arenas, REP_MAX_Y));
+    replay_record_kernel<<<grid, REP_THREADS, 0, c->stream>>>(dE, curmask, rep, ev, R);
+    post_launch("replay_record_kernel");
 }
 
 bool smem_fits(Ctx *c, const EngineDev &hE, int which, int group, int of, std::string *why) {

@@ -254,6 +254,40 @@ struct SlotDev {
     int id_cap;
 };
 
+// The replay recorder (magent_b200_replay_*, replay_phases.h).
+// per-arena replay state, [A] in device memory outside EngineDev and ArenaHdr (a restore copies the header from the
+// snapshot): the episode counter (env_reset and every restore that replaces the arena bump it) and, per group, the rows
+// of the event list the arena's last step wrote (a restore empties it)
+struct RepArena {
+    int episode;
+    int ev_n[MG_MAX_GROUPS];
+};
+
+// one attack row of the event list: rank < 0 where the row's agent executed no attack
+struct RepEvent { int rank, id, x, y; };
+// one agent row of a frame; dir_flags = dir | FLAG_ABSORBED << 8 when absorbed (dir is DIR_NORTH without turn_mode)
+struct RepAgent { int id, x, y; float hp; int dir_flags; };
+
+enum { REP_H_EPISODE = 0, REP_H_WALLS = 1, REP_H_N = 2, REP_H_EV_N = 2 + MG_MAX_GROUPS, REP_HDR_INTS = 32 };
+
+// ints of one frame block: header, cap_total agents, cap_total events, wall bitmap
+struct RepLayout {
+    int cap_total;
+    int wall_words;                          // ceil(W * H / 128) * 4: every frame block stays 16-byte aligned
+    MG_HD long agent_base() const { return REP_HDR_INTS; }
+    MG_HD long event_base() const { return agent_base() + (long)cap_total * (sizeof(RepAgent) / 4); }
+    MG_HD long wall_base() const { return event_base() + (long)cap_total * (sizeof(RepEvent) / 4); }
+    MG_HD long frame_ints() const { return wall_base() + wall_words; }
+};
+
+// the recorder's device control block: frames buffered, frames dropped for want of room, and the CTA ticket of the
+// record kernel (the last CTA to finish advances the counters)
+struct RepCtl {
+    unsigned long long dropped;
+    int n_frames;
+    unsigned ticket;
+};
+
 enum InfoKind { INFO_ID = 0, INFO_POS, INFO_ALIVE, INFO_REWARD, INFO_ACTION_SCATTER, INFO_HP };
 
 }  // namespace mg

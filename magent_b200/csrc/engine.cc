@@ -4,8 +4,11 @@
 #include "nbr_phases.h"
 #include "rule_phases.h"
 #include "slot_phases.h"
+#include "replay_phases.h"
 
+#include <errno.h>
 #include <math.h>
+#include <sys/stat.h>
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -145,6 +148,9 @@ Engine::~Engine() {
     free_device();
     if (d_slot_tab_) be::dfree(bx_, d_slot_tab_);
     if (d_slot_dev_) be::dfree(bx_, d_slot_dev_);
+    for (int id = 0; id < (int)replays_.size(); ++id)
+        if (replays_[id].live) { replays_[id].in_graph = false; replay_free(id); }
+    for (void *p : {(void *)d_rep_, (void *)d_ev_, (void *)d_ev_arenas_}) if (p) be::dfree(bx_, p);
     if (h_feat_stage_) be::host_free(h_feat_stage_);
     if (bx_) be::destroy(bx_);
 }
@@ -472,6 +478,12 @@ void Engine::reset() {                                // GridWorld.cc:72-118, Ma
         where_ = HOST;
     }
     file_ct_++; frame_ct_ = 0;                        // RenderGenerator::next_file (GridWorld.cc:97)
+    if (d_rep_) {                                     // a new episode in every arena for the replay recorders
+        std::vector<RepArena> rep(A_);
+        be::d2h(bx_, rep.data(), d_rep_, sizeof(RepArena) * A_);
+        for (RepArena &r : rep) r.episode++;
+        be::h2d(bx_, d_rep_, rep.data(), sizeof(RepArena) * A_);
+    }
     large_map_ = (long)W_ * H_ > 99 * 99;
     nsep_ = large_map_ ? ((long)W_ * H_ > 1000 * 1000 ? 16 : 8) : 1;
     for (auto &ar : arenas_) {
@@ -1346,7 +1358,8 @@ int Engine::restore_arenas(int id, const int *src, int keep_rng) {
         io_[IO_H2D] += (long long)A_ * 4;
         d_src = st;
     }
-    // the slot rows first: launch_restore rewrites the done words a null src decides by
+    // the slot rows and the recorders' episodes first: launch_restore rewrites the done words a null src decides by
+    if (live_replays()) be::launch_replay_restore(bx_, hE_, d_rep_, d_src);
     if (be::launch_restore_slots) be::launch_restore_slots(bx_, dE_, hE_, d_slot_dev_, sn.slot_tab, sn.slot_id_cap, d_src);
     be::launch_restore(bx_, dE_, hE_, curmask_, sn.dev, d_src, keep_rng ? 1 : 0);
     ++state_version_;
@@ -1681,10 +1694,16 @@ void Engine::step(int *done) {                                        // GridWor
     StepArgs S;
     memset(&S, 0, sizeof S);
     S.curmask = curmask_;
-    S.record_events = first_render_ ? 0 : 1;           // GridWorld.cc:484: only once rendering has started
+    // GridWorld.cc:484: only once rendering has started, or while a replay recorder is live
+    const bool replaying = live_replays() > 0;
+    S.record_events = first_render_ && !replaying ? 0 : 1;
     S.n_order = (int)order_.size();
     for (int k = 0; k < S.n_order; ++k) S.order[k] = order_[k];
     be::launch_step(bx_, dE_, hE_, S, max_agents_per_arena());
+    // the recorded arenas' events, before a cull renumbers the rows (an event list sized for another cap_total is left
+    // alone: replay_record refuses then)
+    if (replaying && hE_.cap_total == ev_stride_)
+        be::launch_replay_events(bx_, dE_, hE_, curmask_, d_rep_, d_ev_, d_ev_arenas_, n_ev_arenas_);
     ++state_version_;
     order_.clear();
     if (be::is_device_ptr(done)) {
@@ -1786,11 +1805,11 @@ void Engine::collect_attack_events() {                // the list GridWorld::ste
         for (int i = 0; i < n; ++i) {
             if (rank[i] < 0) continue;
             const int k = act[i] - t.attack_base;
-            // Map::get_attack_obj (Map.cc:209-221): an attacker neither moves nor turns in the step it attacks
-            int rx, ry, dx, dy;
-            dir_real(hE_.grp[g], dir[i], rx, ry);
-            dir_rot(dir[i], t.att_x_offset + t.attack.dx[k], t.att_y_offset + t.attack.dy[k], dx, dy);
-            evs.push_back({rank[i], id[i], x[i] + rx + dx, y[i] + ry + dy});
+            // an attacker neither moves nor turns in the step it attacks
+            Ev e = {rank[i], id[i], 0, 0};
+            replay_event_cell(hE_.grp[g], dir[i], x[i], y[i], t.att_x_offset + t.attack.dx[k], t.att_y_offset + t.attack.dy[k],
+                              e.x, e.y);
+            evs.push_back(e);
         }
     }
     std::sort(evs.begin(), evs.end(), [](const Ev &p, const Ev &q) { return p.rank < q.rank; });
@@ -1801,9 +1820,9 @@ void Engine::collect_attack_events() {                // the list GridWorld::ste
 void Engine::render_next_file() { file_ct_++; frame_ct_ = 0; }
 
 namespace {
-template <typename T> void print_json(std::ofstream &os, const char *key, T value, bool last = false) {
+template <typename T> void print_json(std::ostream &os, const char *key, T value, bool last = false) {
     os << "\"" << key << "\": " << value;
-    if (last) os << std::endl; else os << "," << std::endl;
+    os << (last ? "\n" : ",\n");
 }
 std::string rgba_string(int r, int g, int b, float alpha) {
     std::stringstream ss;
@@ -1812,75 +1831,267 @@ std::string rgba_string(int r, int g, int b, float alpha) {
 }
 }  // namespace
 
-void Engine::render() {                               // GridWorld.cc:939-949
+void Engine::write_render_config(std::ostream &f) const {             // RenderGenerator::gen_config
     static const int colors[][3] = {{192, 64, 64}, {64, 64, 192}, {64, 192, 64}, {64, 64, 64}};
+    f << "{\n";
+    print_json(f, "width", W_);
+    print_json(f, "height", H_);
+    print_json(f, "static-file", "\"static.map\"");
+    print_json(f, "obstacle-style", rgba_string(127, 127, 127, 1));
+    print_json(f, "dynamic-file-directory", "\".\"");
+    print_json(f, "attack-style", rgba_string(63, 63, 63, 0.8));
+    print_json(f, "minimap-width", 300);
+    print_json(f, "minimap-height", 250);
+    f << "\"group\" : [\n";
+    for (int i = 0; i < G(); i++) {
+        const AgentTypeDef &t = *group_type_[i];
+        const int *c = colors[i % 4];
+        f << "{\n";
+        print_json(f, "height", t.length);
+        print_json(f, "width", t.width);
+        print_json(f, "style", rgba_string(c[0], c[1], c[2], 1));
+        print_json(f, "anchor", "[0, 0]");
+        print_json(f, "max-speed", (int)t.speed);
+        print_json(f, "speed-style", rgba_string(c[0], c[1], c[2], 0.01));
+        print_json(f, "vision-radius", t.view_radius);
+        print_json(f, "vision-angle", t.view_angle);
+        print_json(f, "vision-style", rgba_string(c[0], c[1], c[2], 0.2));
+        print_json(f, "attack-radius", t.attack_radius);
+        print_json(f, "attack-angle", t.attack_angle);
+        print_json(f, "attack-style", rgba_string(c[0], c[1], c[2], 0.1));
+        print_json(f, "broadcast-radius", 1, true);
+        f << (i == G() - 1 ? "}" : "},") << "\n";
+    }
+    f << "]\n}\n";
+}
+
+void Engine::write_render_frame(std::ostream &fout, const std::vector<int> *walls,       // RenderGenerator::render_a_frame
+                                const std::vector<std::vector<RepAgent>> &agents,
+                                const std::vector<AttackEvent> &events) const {
+    if (walls) {
+        fout << "W" << " " << walls->size() << "\n";
+        for (int w : *walls) fout << w % W_ << " " << w / W_ << "\n";
+    }
+    int num_agents = 0;
+    for (int g = 0; g < G(); g++) {
+        num_agents += (int)agents[g].size();
+        if (group_type_[g]->can_absorb)
+            for (const RepAgent &r : agents[g]) if (!(r.dir_flags & (FLAG_ABSORBED << 8))) num_agents--;
+    }
+    fout << "F" << " " << num_agents << " " << (int)events.size() << " " << 0 << "\n";
+    static const int dir2angle[] = {0, 90, 180, 270};
+    for (int g = 0; g < G(); g++) {
+        const AgentTypeDef &t = *group_type_[g];
+        for (const RepAgent &r : agents[g]) {
+            if (t.can_absorb && !(r.dir_flags & (FLAG_ABSORBED << 8))) continue;
+            int hp = std::max(0, int(100 * r.hp / t.hp));
+            hp = std::min(hp, 100);
+            fout << r.id << " " << hp << " " << dir2angle[r.dir_flags & 3] << " " << r.x << " " << r.y << " " << g << "\n";
+        }
+    }
+    for (const AttackEvent &e : events) fout << 0 << " " << e.id << " " << e.x << " " << e.y << "\n";
+}
+
+void Engine::render() {                               // GridWorld.cc:939-949
     if (render_dir_ == "___debug___") return;         // terminal dump of the reference's debug mode: not provided
     if (first_render_) {
         first_render_ = false;
-        std::ofstream f(render_dir_ + "/" + "config.json");           // RenderGenerator::gen_config
-        f << "{" << std::endl;
-        print_json(f, "width", W_);
-        print_json(f, "height", H_);
-        print_json(f, "static-file", "\"static.map\"");
-        print_json(f, "obstacle-style", rgba_string(127, 127, 127, 1));
-        print_json(f, "dynamic-file-directory", "\".\"");
-        print_json(f, "attack-style", rgba_string(63, 63, 63, 0.8));
-        print_json(f, "minimap-width", 300);
-        print_json(f, "minimap-height", 250);
-        f << "\"group\" : [" << std::endl;
-        for (int i = 0; i < G(); i++) {
-            const AgentTypeDef &t = *group_type_[i];
-            const int *c = colors[i % 4];
-            f << "{" << std::endl;
-            print_json(f, "height", t.length);
-            print_json(f, "width", t.width);
-            print_json(f, "style", rgba_string(c[0], c[1], c[2], 1));
-            print_json(f, "anchor", "[0, 0]");
-            print_json(f, "max-speed", (int)t.speed);
-            print_json(f, "speed-style", rgba_string(c[0], c[1], c[2], 0.01));
-            print_json(f, "vision-radius", t.view_radius);
-            print_json(f, "vision-angle", t.view_angle);
-            print_json(f, "vision-style", rgba_string(c[0], c[1], c[2], 0.2));
-            print_json(f, "attack-radius", t.attack_radius);
-            print_json(f, "attack-angle", t.attack_angle);
-            print_json(f, "attack-style", rgba_string(c[0], c[1], c[2], 0.1));
-            print_json(f, "broadcast-radius", 1, true);
-            f << (i == G() - 1 ? "}" : "},") << std::endl;
-        }
-        f << "]" << std::endl << "}" << std::endl;
+        std::ofstream f(render_dir_ + "/" + "config.json");
+        write_render_config(f);
     }
-    if (render_dir_.empty()) return;                  // RenderGenerator::render_a_frame
+    if (render_dir_.empty()) return;
     if (was_reset_ && where_ == DEVICE) to_host(true);
     const HostArena &ar = arenas_[sel_arena_ >= 0 ? sel_arena_ : 0];
     std::ofstream fout(render_dir_ + "/" + "video_" + std::to_string(file_ct_) + ".txt",
                        frame_ct_ == 0 ? std::ios::out : std::ios::app);
-    if (frame_ct_ == 0) {
-        std::vector<int> walls;
+    std::vector<int> walls;
+    if (frame_ct_ == 0)
         for (int i = 0; i < W_ * H_; i++) if (ar.occ[i] == OCC_WALL) walls.push_back(i);
-        fout << "W" << " " << walls.size() << std::endl;
-        for (int w : walls) fout << w % W_ << " " << w / W_ << std::endl;
-    }
-    int num_agents = 0;
+    std::vector<std::vector<RepAgent>> agents(G());
     for (int g = 0; g < G(); g++) {
         const HostGroup &hg = ar.groups[g];
-        num_agents += hg.size();
-        if (group_type_[g]->can_absorb)
-            for (int j = 0; j < hg.size(); j++) if (!(hg.flags[j] & FLAG_ABSORBED)) num_agents--;
+        for (int j = 0; j < hg.size(); j++)
+            agents[g].push_back({hg.id[j], hg.x[j], hg.y[j], hg.hp[j], (hg.dir[j] & 3) | (hg.flags[j] & FLAG_ABSORBED ? FLAG_ABSORBED << 8 : 0)});
     }
-    fout << "F" << " " << num_agents << " " << (int)attack_events_.size() << " " << 0 << std::endl;
-    for (int g = 0; g < G(); g++) {
-        const HostGroup &hg = ar.groups[g];
-        const AgentTypeDef &t = *group_type_[g];
-        for (int j = 0; j < hg.size(); j++) {
-            if (t.can_absorb && !(hg.flags[j] & FLAG_ABSORBED)) continue;
-            int hp = std::max(0, int(100 * hg.hp[j] / t.hp));
-            hp = std::min(hp, 100);
-            static const int dir2angle[] = {0, 90, 180, 270};
-            fout << hg.id[j] << " " << hp << " " << dir2angle[hg.dir[j] & 3] << " " << hg.x[j] << " " << hg.y[j] << " " << g << std::endl;
-        }
-    }
-    for (const AttackEvent &e : attack_events_) fout << 0 << " " << e.id << " " << e.x << " " << e.y << std::endl;
+    write_render_frame(fout, frame_ct_ == 0 ? &walls : nullptr, agents, attack_events_);
     if (frame_ct_++ > frame_per_file_) { frame_ct_ = 0; file_ct_++; }
+}
+
+// ---------------------------------------------------------------------------------------------
+// replay recorders (replay_phases.h): frames of chosen arenas gathered on the device without synchronisation or
+// allocation, so that recording can sit inside a captured step loop; replay_write formats them as env_render would.
+int Engine::live_replays() const {
+    int n = 0;
+    for (const ReplayRec &r : replays_) n += r.live ? 1 : 0;
+    return n;
+}
+
+// the arenas whose attack events the step collects: the union of the live recorders' (read by the event kernel from
+// device memory, so a captured step sees the set shrink when a recorder outside the graph is freed)
+void Engine::update_ev_arenas() {
+    std::vector<int> list(A_, -1);
+    std::vector<char> in(A_, 0);
+    n_ev_arenas_ = 0;
+    for (const ReplayRec &r : replays_)
+        if (r.live)
+            for (int a : r.arenas) if (!in[a]) { in[a] = 1; list[n_ev_arenas_++] = a; }
+    be::h2d(bx_, d_ev_arenas_, list.data(), (size_t)A_ * 4);
+}
+
+int Engine::replay_new(const int *arenas, int n_arenas, int max_frames) {
+    if (bx_ && be::capturing(bx_)) return refuse("replay_new allocates device memory: not possible while a CUDA graph is being captured");
+    if (graph_captured_)
+        return refuse("replay_new after this game captured a CUDA graph: steps captured without a live recorder do not record "
+                      "attack events, so create recorders before capturing");
+    if (!was_reset_) return refuse("replay_new before reset");
+    if (!be::launch_replay_events || !be::launch_replay_restore || !be::launch_replay_record)
+        return refuse("the %s backend has no replay kernels", be::name());
+    if (!arenas || n_arenas < 1) return refuse("replay_new: the arena list is empty");
+    if (max_frames < 1) return refuse("replay_new: max_frames = %d, must be >= 1", max_frames);
+    std::vector<char> seen(A_, 0);
+    for (int k = 0; k < n_arenas; ++k) {
+        const int a = arenas[k];
+        if (a < 0 || a >= A_) return refuse("replay_new: arena %d is outside [0, %d)", a, A_);
+        if (seen[a]) return refuse("replay_new: arena %d is listed twice", a);
+        seen[a] = 1;
+    }
+    to_device();
+    ReplayRec r;
+    r.arenas.assign(arenas, arenas + n_arenas);
+    r.max_frames = max_frames;
+    r.cap = cap_;
+    r.W = W_; r.H = H_;
+    r.L.cap_total = hE_.cap_total;
+    r.L.wall_words = (int)(((long)W_ * H_ + 127) / 128 * 4);      // a multiple of 4: every frame block starts 16-byte aligned
+    r.file_ct.assign(n_arenas, 0);
+    r.frame_ct.assign(n_arenas, 0);
+    r.walls.assign(n_arenas, {});
+    const size_t frame_bytes = (size_t)r.L.frame_ints() * 4;
+    r.frames = (int *)be::dmalloc(bx_, frame_bytes * n_arenas * max_frames);
+    r.d_arenas = (int *)be::dmalloc(bx_, (size_t)n_arenas * 4);
+    be::h2d(bx_, r.d_arenas, arenas, (size_t)n_arenas * 4);
+    r.last_ep = (int *)be::dmalloc(bx_, (size_t)n_arenas * 4);
+    be::dmemset(bx_, r.last_ep, 0xff, (size_t)n_arenas * 4);      // -1: no frame yet (episodes count up from 0)
+    r.ctl = (RepCtl *)be::dmalloc(bx_, sizeof(RepCtl));
+    be::dmemset(bx_, r.ctl, 0, sizeof(RepCtl));
+    if (!d_rep_) {
+        d_rep_ = (RepArena *)be::dmalloc(bx_, sizeof(RepArena) * A_);
+        be::dmemset(bx_, d_rep_, 0, sizeof(RepArena) * A_);
+        d_ev_arenas_ = (int *)be::dmalloc(bx_, (size_t)A_ * 4);
+    }
+    // no events are known until the next step when none were being collected, or for a list of another width
+    if (!live_replays() || ev_stride_ != hE_.cap_total) {
+        if (ev_stride_ != hE_.cap_total) {
+            if (d_ev_) be::dfree(bx_, d_ev_);
+            ev_stride_ = hE_.cap_total;
+            d_ev_ = (RepEvent *)be::dmalloc(bx_, sizeof(RepEvent) * std::max<size_t>((size_t)A_ * ev_stride_, 1));
+        }
+        std::vector<RepArena> rep(A_);
+        be::d2h(bx_, rep.data(), d_rep_, sizeof(RepArena) * A_);
+        for (RepArena &x : rep) for (int &n : x.ev_n) n = 0;
+        be::h2d(bx_, d_rep_, rep.data(), sizeof(RepArena) * A_);
+    }
+    r.live = true;
+    replays_.push_back(r);                            // ids are never reused: a freed id stays unknown
+    update_ev_arenas();
+    return (int)replays_.size() - 1;
+}
+
+int Engine::replay_record(int id) {
+    if (id < 0 || id >= (int)replays_.size() || !replays_[id].live) return refuse("unknown or freed replay id %d", id);
+    ReplayRec &r = replays_[id];
+    to_device();
+    if (r.cap != cap_ || r.L.cap_total != hE_.cap_total || ev_stride_ != hE_.cap_total || r.W != W_ || r.H != H_)
+        return refuse("replay_record: the per-arena agent bound grew past what replay %d's frames were sized for "
+                      "(create a new recorder)", id);
+    be::RepRecord R;
+    R.arenas = r.d_arenas;
+    R.n_arenas = (int)r.arenas.size();
+    R.max_frames = r.max_frames;
+    R.L = r.L;
+    R.frames = r.frames;
+    R.last_ep = r.last_ep;
+    R.ctl = r.ctl;
+    be::launch_replay_record(bx_, dE_, hE_, curmask_, d_rep_, d_ev_, R);
+    if (be::capturing(bx_)) r.in_graph = true;
+    return 0;
+}
+
+static bool make_dir(const std::string &d) { return mkdir(d.c_str(), 0777) == 0 || errno == EEXIST; }
+
+int Engine::replay_write(int id, const char *dir, long long *dropped) {
+    if (id < 0 || id >= (int)replays_.size() || !replays_[id].live) return refuse("unknown or freed replay id %d", id);
+    if (be::capturing(bx_)) return refuse("replay_write synchronises: not possible while a CUDA graph is being captured");
+    if (!dir) return refuse("replay_write: no directory");
+    ReplayRec &r = replays_[id];
+    const int nk = (int)r.arenas.size();
+    std::vector<std::string> sub(nk);
+    if (!make_dir(dir)) return refuse("replay_write: cannot create %s", dir);
+    for (int k = 0; k < nk; ++k) {
+        sub[k] = std::string(dir) + "/arena_" + std::to_string(r.arenas[k]);
+        if (!make_dir(sub[k])) return refuse("replay_write: cannot create %s", sub[k].c_str());
+    }
+    be::sync(bx_);
+    RepCtl ctl;
+    be::d2h(bx_, &ctl, r.ctl, sizeof ctl);
+    const long fi = r.L.frame_ints();
+    std::vector<int> buf((size_t)ctl.n_frames * nk * fi);
+    be::d2h(bx_, buf.data(), r.frames, buf.size() * 4);
+    const int Gn = G();
+    std::vector<std::vector<RepAgent>> agents(Gn);
+    std::vector<AttackEvent> events;
+    std::vector<RepEvent> evs;
+    for (int k = 0; k < nk; ++k) {
+        std::ofstream cfg(sub[k] + "/config.json");
+        write_render_config(cfg);
+        std::ofstream out;
+        int open_file = 0;
+        for (int f = 0; f < ctl.n_frames; ++f) {
+            const int *F = buf.data() + ((size_t)f * nk + k) * fi;
+            if (F[REP_H_WALLS]) {                     // the first frame of an episode opens a file, unless a split just did
+                if (r.file_ct[k] == 0 || r.frame_ct[k] != 0) r.file_ct[k]++;
+                r.frame_ct[k] = 0;
+                std::vector<int> &w = r.walls[k];
+                w.clear();
+                for (int q = 0; q < r.L.wall_words; ++q)
+                    for (unsigned bits = (unsigned)F[r.L.wall_base() + q]; bits; bits &= bits - 1)
+                        w.push_back(q * 32 + __builtin_ctz(bits));
+            }
+            if (open_file != r.file_ct[k]) {
+                out.close();
+                out.open(sub[k] + "/video_" + std::to_string(r.file_ct[k]) + ".txt", r.frame_ct[k] == 0 ? std::ios::out : std::ios::app);
+                if (!out) return refuse("replay_write: cannot write %s/video_%d.txt", sub[k].c_str(), r.file_ct[k]);
+                open_file = r.file_ct[k];
+            }
+            const RepAgent *ag = (const RepAgent *)(F + r.L.agent_base());
+            const RepEvent *ev = (const RepEvent *)(F + r.L.event_base());
+            evs.clear();
+            for (int g = 0, base = 0; g < Gn; base += r.cap[g], ++g) {        // rows at the flat offsets of r.cap
+                agents[g].assign(ag + base, ag + base + F[REP_H_N + g]);
+                for (int i = 0; i < F[REP_H_EV_N + g]; ++i) if (ev[base + i].rank >= 0) evs.push_back(ev[base + i]);
+            }
+            std::sort(evs.begin(), evs.end(), [](const RepEvent &p, const RepEvent &q) { return p.rank < q.rank; });
+            events.clear();
+            for (const RepEvent &e : evs) events.push_back({e.id, e.x, e.y});
+            write_render_frame(out, r.frame_ct[k] == 0 ? &r.walls[k] : nullptr, agents, events);
+            if (r.frame_ct[k]++ > frame_per_file_) { r.frame_ct[k] = 0; r.file_ct[k]++; }
+        }
+        if (out.is_open() && !out.flush()) return refuse("replay_write: cannot write %s", sub[k].c_str());
+    }
+    if (dropped) *dropped = (long long)ctl.dropped;
+    be::dmemset(bx_, r.ctl, 0, sizeof(RepCtl));
+    return ctl.n_frames;
+}
+
+int Engine::replay_free(int id) {
+    if (id < 0 || id >= (int)replays_.size() || !replays_[id].live) return refuse("unknown or freed replay id %d", id);
+    ReplayRec &r = replays_[id];
+    if (r.in_graph) return refuse("replay %d is recorded into from inside a CUDA graph: it lives as long as the game", id);
+    if (be::capturing(bx_)) return refuse("replay_free is not possible while a CUDA graph is being captured");
+    for (void *p : {(void *)r.frames, (void *)r.d_arenas, (void *)r.last_ep, (void *)r.ctl}) be::dfree(bx_, p);
+    r = ReplayRec();
+    update_ev_arenas();
+    return 0;
 }
 
 void Engine::sync() { if (bx_) be::sync(bx_); }
@@ -1895,6 +2106,7 @@ void Engine::graph_begin() {
     capture_floor_ = std::any_of(floor.begin(), floor.end(), [](int v) { return v > 0; });
     if (capture_floor_) raise_counts(floor);
     if (!be::capture_begin(bx_)) fatal("this backend has no CUDA graph support");
+    graph_captured_ = true;
 }
 int Engine::graph_end() {
     const int id = be::capture_end(bx_);

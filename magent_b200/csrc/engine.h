@@ -6,6 +6,7 @@
 // uploads the image to HBM and from then on every step-loop call is a kernel launch (backend.h).
 #pragma once
 #include <stdint.h>
+#include <iosfwd>
 #include <map>
 #include <string>
 #include <vector>
@@ -87,6 +88,23 @@ struct ArenaSnapshot {
     std::vector<void *> allocs;
 };
 
+// a replay recorder (Engine::replay_new): frames of chosen arenas buffered in its own device memory, written out in the
+// reference viewer's format by Engine::replay_write
+struct ReplayRec {
+    bool live = false;
+    bool in_graph = false;              // recorded into a CUDA graph: lives as long as the engine
+    std::vector<int> arenas;
+    int max_frames = 0;
+    std::vector<int> cap;               // [G] per-arena capacity the frames are sized for
+    RepLayout L = {0, 0};
+    int W = 0, H = 0;
+    int *d_arenas = nullptr, *frames = nullptr, *last_ep = nullptr;
+    RepCtl *ctl = nullptr;
+    // writer state per recorded arena: the open file (0: none yet), frames in it, the walls of its episode
+    std::vector<int> file_ct, frame_ct;
+    std::vector<std::vector<int>> walls;
+};
+
 struct SymbolDef { int group = 0, index = 0; };
 struct NodeDef { int op = OP_NULL; std::vector<int> raw; };
 struct RuleDef { int on = 0; std::vector<int> recv; std::vector<float> values; bool is_terminal = false, auto_value = false; };
@@ -165,6 +183,12 @@ public:
     int rule_actions(int group, int target, int policy, unsigned long long seed);
     int get_rule_actions(int group, int target, int policy, unsigned long long seed, int *act);
     int get_rule_actions_slots(int group, int target, int policy, unsigned long long seed, int *act);
+    // replay recorder (replay_phases.h): record frames of chosen arenas on the device, write them as env_render would.
+    // -1 and the last error when refused.
+    int replay_new(const int *arenas, int n_arenas, int max_frames);
+    int replay_record(int id);
+    int replay_write(int id, const char *dir, long long *dropped);
+    int replay_free(int id);
     int get_counters(long long *out, int cap);
     void sync();
     void get_io_stats(long long *out, int cap);      // bytes so far: device->host over PCIe, host->device, written by host threads
@@ -205,6 +229,25 @@ private:
     struct AttackEvent { int id, x, y; };
     std::vector<AttackEvent> attack_events_;
     void collect_attack_events();
+    // the one formatter of env_render and replay_write: config.json, and one frame (walls: the wall cells when the frame
+    // opens a file, else null; agents: every row of each group, in row order)
+    void write_render_config(std::ostream &os) const;
+    void write_render_frame(std::ostream &os, const std::vector<int> *walls,
+                            const std::vector<std::vector<RepAgent>> &agents,
+                            const std::vector<AttackEvent> &events) const;
+    // replay recorders: the per-arena episode counters and event-list counts ([A], outside EngineDev and ArenaHdr, kept
+    // across re-allocations), the event list ([A][ev_stride_] RepEvent, sized for cap_total at the last replay_new), the
+    // arenas whose events the step collects ([A], the union of the live recorders', n_ev_arenas_ of them), and whether
+    // this game has ever captured a CUDA graph (steps captured without a live recorder cannot record events)
+    std::vector<ReplayRec> replays_;
+    RepArena *d_rep_ = nullptr;
+    RepEvent *d_ev_ = nullptr;
+    int ev_stride_ = 0;
+    int *d_ev_arenas_ = nullptr;
+    int n_ev_arenas_ = 0;
+    bool graph_captured_ = false;
+    int live_replays() const;
+    void update_ev_arenas();
 
     // host image
     std::vector<HostArena> arenas_;

@@ -161,6 +161,14 @@ MG_API int magent_b200_free_snapshot(EnvHandle game, int snapshot) { return E(ga
 MG_API int magent_b200_restore_arenas(EnvHandle game, int snapshot, const int *src, int keep_rng) {
     return E(game)->restore_arenas(snapshot, src, keep_rng);
 }
+MG_API int magent_b200_replay_new(EnvHandle game, const int *arenas, int n_arenas, int max_frames) {
+    return E(game)->replay_new(arenas, n_arenas, max_frames);
+}
+MG_API int magent_b200_replay_record(EnvHandle game, int replay) { return E(game)->replay_record(replay); }
+MG_API int magent_b200_replay_write(EnvHandle game, int replay, const char *dir, long long *dropped) {
+    return E(game)->replay_write(replay, dir, dropped);
+}
+MG_API int magent_b200_replay_free(EnvHandle game, int replay) { return E(game)->replay_free(replay); }
 MG_API int magent_b200_get_arena_done(EnvHandle game, int *out) { return E(game)->get_arena_done(out); }
 MG_API int magent_b200_get_counters(EnvHandle game, long long *out, int capacity) { return E(game)->get_counters(out, capacity); }
 MG_API long long magent_b200_launch_count(void) { return mg::be::launch_count(); }

@@ -560,6 +560,30 @@ class GridWorld(Environment):
         self._check(self._lib.magent_b200_restore_arenas(self.game, int(snapshot), ptr, 1 if keep_rng else 0),
                     "restore_arenas")
 
+    # ---- replay recorder: watch chosen arenas of a device-resident loop in the reference viewer's format
+    def new_replay(self, arenas, max_frames):
+        """a recorder of the listed arenas with room for max_frames frames on the device; returns its id.  Make it
+        before capturing any CUDA graph: steps captured without a live recorder record no attack events."""
+        arr = np.ascontiguousarray(np.asarray(arenas, dtype=np.int32).reshape(-1))
+        return self._check(self._lib.magent_b200_replay_new(self.game, arr.ctypes.data, int(arr.size), int(max_frames)),
+                           "new_replay")
+
+    def record_replay(self, replay):
+        """append one frame of every arena of the recorder, the frame render() would write for it; waits for nothing
+        and can be recorded into a CUDA graph (capture_graph)"""
+        self._check(self._lib.magent_b200_replay_record(self.game, int(replay)), "record_replay")
+
+    def write_replay(self, replay, directory):
+        """write the buffered frames as directory/arena_<a>/config.json and video_<k>.txt and empty the buffer;
+        returns (frames written per arena, frames dropped for want of room since the last write)"""
+        dropped = ctypes.c_longlong(0)
+        n = self._check(self._lib.magent_b200_replay_write(self.game, int(replay), os.fsencode(directory),
+                                                           ctypes.addressof(dropped)), "write_replay")
+        return n, int(dropped.value)
+
+    def free_replay(self, replay):
+        self._check(self._lib.magent_b200_replay_free(self.game, int(replay)), "free_replay")
+
     def get_arena_done_torch(self, out=None):
         """per-arena done flags of the last step into an int32 CUDA tensor (num_arenas,); nothing waits for the host"""
         import torch
